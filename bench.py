@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — agent-steps/sec of the batched F1TENTH hot path on N B200s (weak scaling), with the
+"""bench.py — agent-steps/sec of the batched F1TENTH hot path on N H100s (weak scaling), with the
 roofline of the ray-march kernel and the CPU baseline beside it.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3|cfg2|cfg2x2|cfg5_B] [--no-extras]
+    python bench.py ... --dump-outputs DIR    # also write what the last timed step computed, as DIR/<name>.npy
     python bench.py --impl reference ...      # the reference's own numba path (oracle/_ref), one process per host core
     torchrun ... bench.py --gpus N ...        # one rank per GPU; envs shard, no data-path collective
 
@@ -37,7 +38,7 @@ def _baseline_metric():
         with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'BASELINE.json')) as f:
             return json.load(f)['metric']
     except Exception:
-        return 'agent-steps/sec (1080-beam scan) at 1/2/4/8 B200 vs reference numba CPU'
+        return 'agent-steps/sec (1080-beam scan) at 1/2/4/8 H100 vs reference numba CPU'
 
 
 METRIC = _baseline_metric()
@@ -61,6 +62,7 @@ EXTRA_WORKLOADS = ['cfg2', 'cfg2x2', 'cfg5_270', 'cfg5_540', 'cfg5_1080', 'cfg5_
 POSE_GAP = 23          # second agent 23 waypoints (~4.6 m) behind (SURVEY 8d)
 SEED = 12345
 FLUSH_BYTES = 256 << 20
+DUMP_BYTES = 48 << 20  # --dump-outputs: total size cap (under 64 MB); the scan block is a fixed, seeded sample of agent rows above it
 
 
 def config_dict(workload, world, sample=None):
@@ -80,7 +82,7 @@ def measured_peak():
         with open(p) as f:
             return float(json.load(f)['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
     except Exception:
-        return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+        return 3350.0, 'fallback (H100 SXM data sheet, 3.35 TB/s)'
 
 
 def ncu_traffic(workload):
@@ -302,9 +304,28 @@ def run_reference(args):
 
 
 # --------------------------------------------------------------------------------------- GPU side
+def step_outputs(sim):
+    """What a caller of the timed tick receives (state, scans, collisions, done, lap times and counts) as float32 / float64
+    host arrays.  Scans larger than the dump budget are cut to a fixed, seeded sample of agent rows (`scan_rows`)."""
+    import torch
+    NA, B = sim.num_envs * sim.num_agents, sim.num_beams
+    out = {'state': sim.state.cpu().numpy(), 'collisions': sim.collisions.cpu().numpy(),
+           'done': sim.done.cpu().numpy().astype(np.float32), 'lap_times': sim.lap_times.cpu().numpy(),
+           'lap_counts': sim.lap_counts.cpu().numpy()}
+    budget = DUMP_BYTES - sum(a.nbytes for a in out.values())
+    scans = sim.scans
+    if NA * B * 4 > budget:
+        rows = np.sort(np.random.default_rng(SEED).choice(NA, budget // (B * 4 + 8), replace=False))
+        out['scan_rows'] = rows.astype(np.float64)
+        scans = scans[torch.from_numpy(rows).to(scans.device)]
+    out['scans'] = scans.cpu().numpy()
+    return out
+
+
 def measure_workload(name, K, W, world, rank, dev, dmap, Ke, prof_ticks, f110, torch, dist, reduce_max_scalar,
-                     sampler_index=None, packed=False):
-    """One workload on this rank's GPU -> dict(value, ms_per_step, e2e, roofline, clocks, ...) (whole-job figures)."""
+                     sampler_index=None, packed=False, dump=False):
+    """One workload on this rank's GPU -> dict(value, ms_per_step, e2e, roofline, clocks, ...) (whole-job figures);
+    with `dump`, also `outputs`: step_outputs() right after the last timed step."""
     w = WORKLOADS[name]
     N, A, B = w['num_envs'], w['num_agents'], w['num_beams']
     NA = N * A
@@ -355,6 +376,7 @@ def measure_workload(name, K, W, world, rank, dev, dmap, Ke, prof_ticks, f110, t
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - wall0
     clocks = sampler.stop() if sampler else None
+    outputs = step_outputs(sim) if dump else None
     if world > 1:
         dist.barrier()
     step_ms = np.array([a.elapsed_time(b) for a, b in zip(ev0, ev1)])
@@ -391,7 +413,7 @@ def measure_workload(name, K, W, world, rank, dev, dmap, Ke, prof_ticks, f110, t
                 'kernel_ms': {'k_dynamics': kms[0], 'k_march': kms[1], 'k_tail': kms[2]},
                 'march_share_of_step': kms[1] / max(kms.sum(), 1e-12),
                 'note': 'the 20.5 MB DT table is L2/L1-resident, so real DRAM traffic is far below the '
-                        'algorithmic bytes; see profiles/ for ncu DRAM and L2 throughput'}
+                        'algorithmic bytes'}
 
     # ---- end to end through the host-buffer API (pipelined: the D2H of tick t overlaps the compute of tick t+1)
     # the caller's actions live in host memory; they are written into the pinned action buffer with a plain
@@ -448,7 +470,7 @@ def measure_workload(name, K, W, world, rank, dev, dmap, Ke, prof_ticks, f110, t
                            'device by f110_pack_scans_u24 inside f110_step_host_async; everything else as in e2e'}
     del sets, sim, flush
     torch.cuda.empty_cache()
-    return {'value': value, 'e2e_packed_u24': e2e_u24, 'ms_per_step': dev_ms_total / K, 'steps': K, 'warmup': W, 'e2e': e2e, 'roofline': roofline,
+    return {'value': value, 'outputs': outputs, 'e2e_packed_u24': e2e_u24, 'ms_per_step': dev_ms_total / K, 'steps': K, 'warmup': W, 'e2e': e2e, 'roofline': roofline,
             'clocks': clocks, 'wall_ms_per_step_incl_flush': 1e3 * wall / K, 'num_envs_per_gpu': N, 'num_agents': A,
             'num_beams': B,
             'step_ms_percentiles': {'p5': float(np.percentile(step_ms, 5)), 'p50': float(np.percentile(step_ms, 50)),
@@ -488,7 +510,12 @@ def run_b200(args):
     dmap = f110.DeviceMap.from_yaml(f110.maps.resolve_map_path('example_map'), '.png', dev)
     common = dict(world=world, rank=rank, dev=dev, dmap=dmap, f110=f110, torch=torch, dist=dist,
                   reduce_max_scalar=reduce_max_scalar)
-    main = measure_workload(args.workload, K, W, Ke=min(K, 200), prof_ticks=20, sampler_index=local_rank, packed=True, **common)
+    main = measure_workload(args.workload, K, W, Ke=min(K, 200), prof_ticks=20, sampler_index=local_rank, packed=True,
+                            dump=bool(args.dump_outputs) and rank == 0, **common)
+    if main['outputs'] is not None:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, a in main['outputs'].items():
+            np.save(os.path.join(args.dump_outputs, name + '.npy'), a)
 
     # optional NCCL observation all-gather for a single-process trainer (SURVEY 8e), timed OFF the step path
     gather = None
@@ -571,7 +598,11 @@ def main():
     ap.add_argument('--cpu-seconds', type=float, default=10.0)
     ap.add_argument('--no-cpu', action='store_true')
     ap.add_argument('--no-extras', action='store_true', help='skip the other BASELINE configs (1 GPU only)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step of the main workload as DIR/<name>.npy (rank 0)')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     if args.warmup < 3:
         args.warmup = 3
     if args.impl == 'reference':

@@ -1,9 +1,9 @@
-"""f1tenth_gym_b200 — B200-native batched F1TENTH simulator hot path.
+"""f1tenth_gym_b200 — batched F1TENTH simulator hot path for the H100.
 
 Drop-in for the per-tick path of f1tenth/f1tenth_gym (Simulator.step: pid + RK4 single-track dynamics,
 1080-beam lidar ray-march on the distance-transform grid, iTTC, opponent ray-cast, GJK collision)
 behind the reference's own Python surface (F110Env / Simulator / ScanSimulator2D and the @njit kernel
-names).  Compute happens only in libf110_b200.so (hand-written sm_100a CUDA behind a C ABI).
+names).  Compute happens only in libf110_b200.so (hand-written sm_90a CUDA behind a C ABI).
 """
 from .simulator import Integrator, Simulator, DeviceMap, DeviceBeams   # noqa: F401
 from .env import F110Env                                              # noqa: F401

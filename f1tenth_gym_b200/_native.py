@@ -1,7 +1,7 @@
 """ctypes binding of libf110_b200.so (C ABI declared in include/f110_b200.h).
 
 There is NO fallback: if the shared library is missing or fails to load, every product entry point
-raises.  Build it with `python -m f1tenth_gym_b200.build` (nvcc, sm_100a) — __graft_entry__.build()
+raises.  Build it with `python -m f1tenth_gym_b200.build` (nvcc, sm_90a) — __graft_entry__.build()
 does that.
 """
 import ctypes as C

@@ -1,4 +1,4 @@
-"""Build libf110_b200.so in-tree with nvcc for sm_100a.   python -m f1tenth_gym_b200.build [--force]
+"""Build libf110_b200.so in-tree with nvcc for sm_90a (H100).   python -m f1tenth_gym_b200.build [--force]
 
 -fmad=false: the reference's numba path performs `x += d*c` as two roundings; FMA contraction would
 change which DT cell a ray lands in (SURVEY.md 7.1).  -lineinfo keeps the ncu source page usable.
@@ -19,7 +19,7 @@ def deps():
     import glob
     return sorted(glob.glob(os.path.join(CSRC, '*.cu')) + glob.glob(os.path.join(CSRC, '*.cuh')) +
                   glob.glob(os.path.join(INCLUDE, '*.h')) + [os.path.abspath(__file__)])
-NVCC_FLAGS = ['-shared', '-Xcompiler', '-fPIC', '-gencode', 'arch=compute_100a,code=sm_100a', '-O3',
+NVCC_FLAGS = ['-shared', '-Xcompiler', '-fPIC', '-gencode', 'arch=compute_90a,code=sm_90a', '-O3',
               '-lineinfo', '-fmad=false', '-std=c++17']
 
 

@@ -9,7 +9,7 @@
 //   k_tail         warp per agent       GJK vs. the other agents of the env, wall-hit state zeroing, opponent ray-cast inside the
 //                                       blocked-view window, collisions obs, then lap logic and auto-reset per env
 //                                       (k_finalize = the same without the env-level part, for f110_step)
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false (no FMA contraction).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (no FMA contraction).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -80,7 +80,7 @@ static BeamView make_view(const f110_beams *b) {
 // extra blocks of k_dynamics (it only reads march_cost, which the reset kernels mark as unknown).
 #define F110_ORDER_ITEMS_PER_THREAD 8
 __device__ __forceinline__ void build_march_order(const f110_sim &s, unsigned first_block, unsigned items) {
-    // Round 2 (profiles/r2/dynamics_cfg3_line_hot.txt: the builder was 65 % of k_dynamics' instructions at cfg3 -- 24 ballots
+    // Round 2 (the builder was most of k_dynamics' instructions at cfg3 -- 24 ballots
     // and up to 24 shared atomics per thread, a runtime division per item): a thread owns EIGHT CONSECUTIVE items, so
     //   * one division per thread (the items after the first step (agent, slice) incrementally),
     //   * the neighbours of an item are the thread's own registers (only the two ends are extra loads: 10 loads, not 24),
@@ -654,7 +654,7 @@ __global__ void __launch_bounds__(MAXT, MINB) k_tail(f110_sim s, BeamView bv, in
 // ------------------------------------------------------------------------------------ k_tail2 (2 <= A <= 4)
 // Same results as k_tail, reorganised (round 2).  ncu on k_tail at 16384 x 2: 1317 warp-instructions per agent, most of them the
 // per-agent SCALAR prologue (opponent vertices, six atan2, asin, sqrt, nearest-beam searches) that all 32 lanes of the agent's
-// warp execute redundantly (profiles/r2/finalize_cfg3_line_hot.txt).  Here a block owns EPB whole envs and works in three phases:
+// warp execute redundantly.  Here a block owns EPB whole envs and works in three phases:
 //   1. one THREAD per (ego, opponent) pair does the scalar prologue -- 32 pairs per warp instead of one -- and leaves a task
 //      record in shared memory; one thread per agent also does the wall-hit zeroing, GJK and the collisions observation;
 //   2. one WARP per ego walks its tasks and ray-casts the windows beam-parallel (the same loop as finalize_agent);
@@ -968,20 +968,20 @@ static int num_sms() {
     if (n <= 0) {
         int dev = 0;
         if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-            n = 148;
+            n = 132;                          // H100 SXM
     }
     return n;
 }
 
-// A/B switch for measurements (profiles/r2/README.md; f110_debug_set_variant or F110_MARCH_VARIANT): 0 = default (k_march_lean,
+// A/B switch for measurements (f110_debug_set_variant or F110_MARCH_VARIANT): 0 = default (k_march_lean,
 // fp64 table, half of the queue dynamic); 66 / 60 / 61 = static dealing with 4 x 512 / 2 x 1024 / 8 x 256 threads per SM;
 // 40 / 41 / 42 = dynamic with 4 x 512 / 3 x 512 / 2 x 1024; 20 / 22 = rank-coded table + shared LUT; 21 = 48 warps/SM;
 // 30 / 31 = TMA tile 128 / 160 cells; 62-65 = thread-block clusters sharing a ticket counter; 1 / 6 = round-1 persistent kernel
 // (fp64 / coded); 7 / 9 = no queue (block per 64-beam tile); 13 = the literal k_raymarch
 static int g_variant = -1, g_chunk = -1;
 // Dynamic second half of the queue (k_march_lean<DYN>): every block gets g_dyn_pct % of its fair share dealt statically and claims
-// the rest in runs from one global counter, g_dyn_ahead runs ahead of their use.  50 % / 4 is the measured optimum (cfg3 march
-// 419 -> 407 us, cfg2x2 116 -> 113.6, cfg2 68.5 -> 68.1; profiles/r2/ab_march_11..13_*.jsonl): the default of variant 0.
+// the rest in runs from one global counter, g_dyn_ahead runs ahead of their use.  50 % / 4 was the measured optimum at cfg3, cfg2x2
+// and cfg2: the default of variant 0.
 static int g_dyn_pct = 50, g_dyn_ahead = 4;
 static int g_ipt[4] = {-1, -1, -1, 255};  // log2(entries per ticket): very heavy, heavy, light runs, dynamic tail (255 = by the class it starts in); -1 = by queue length
 static int rm_variant() {
@@ -1027,9 +1027,8 @@ static void launch_persistent(const MarchK &k, const MarchQueue &mq, unsigned bl
 
 // Launch with the programmatic-stream-serialization attribute (PDL) when enabled: the kernel may become resident before
 // its predecessor in the stream has finished and synchronises itself with pdl_wait().
-// measured (profiles/r2/ab_march_5_pdl_tail.jsonl): inside a CUDA graph PDL wins nothing (cfg2 85.9 vs 86.0-88.0 us, cfg3 563-573 vs
-// 560-569 us), so it is off by default and kept as a switch (f110_debug_set_pdl); k_tail is fastest with the 64-register
-// budget (occupancy beats spills: cfg3 560.0 / 565.1 / 569.3 us for 64 / 96 / 128 registers)
+// measured: inside a CUDA graph PDL wins nothing, so it is off by default and kept as a switch (f110_debug_set_pdl); k_tail
+// is fastest with the 64-register budget (occupancy beats spills against 96 / 128 registers)
 static int g_pdl = 0;
 static int g_tail_minb = 8;
 static int g_tail2_threads = F110_TAIL2_THREADS, g_tail2_agents = 64;    // block shape of k_tail2 (f110_debug_set_tail2)
@@ -1096,9 +1095,8 @@ static void launch_lean(const LeanK &q, const MarchQueue &mq, unsigned sms, bool
         if (getenv("F110_DEBUG")) fprintf(stderr, "f110: cluster variant %d does not fit, using the default launch\n", v);
     }
     // Block shape at the same 64 warps/SM.  Two 1024-thread blocks per SM (32 warps share a ticket counter, the queue is dealt
-    // to half as many blocks) beat four 512-thread blocks whenever a block gets enough items -- cfg3 march 443 -> 420 us,
-    // cfg5_2160 819 -> 761, cfg2x2 120.2 -> 116.2 -- and lose when it does not: cfg2 (470 items per big block) 68.2 -> 70.5 us
-    // (profiles/r2/ab_march_7_*.jsonl, ab_march_8_*.jsonl).  Variant 60 / 61 / 66 force 2 x 1024 / 8 x 256 / 4 x 512.
+    // to half as many blocks) beat four 512-thread blocks whenever a block gets enough items (cfg3, cfg5_2160, cfg2x2) and
+    // lose when it does not (cfg2, 470 items per big block).  Variant 60 / 61 / 66 force 2 x 1024 / 8 x 256 / 4 x 512.
     const int v = rm_variant();
     const bool big = (v == 60) || (v != 61 && v != 66 && v != 44 && v != 21 && v != 22 && !dyn && !coded && !occ3 &&
                                    (unsigned long long)mq.items >= 700ull * 2ull * (unsigned long long)sms);
@@ -1132,12 +1130,12 @@ static void launch_lean(const LeanK &q, const MarchQueue &mq, unsigned sms, bool
         if (occ3) launch_lean_t<0, true, false, 3, true>(q, mq, sms * 3u, noise, count, st);
         else if (v == 40) launch_lean_t<0, true, false, 4, true>(q, mq, sms * 4u, noise, count, st);       // one entry per ticket, compile-time
         // Long queues (>= 72 entries per warp: cfg3, the beam sweep): four entries per ticket throughout, fixed at compile time --
-        // cfg3 march 368 us against 378 with the very heavy runs dealt one or two entries at a time, 407 with one entry per
-        // ticket everywhere.  Shorter queues: ticket size by the class of the run (dyn_queue_position_zoned), which is what
-        // keeps four very heavy entries from landing on one warp (uniform 4: cfg2x2 139 us instead of 112, cfg2 122 instead of 68).
-        // Medium queues (27..72 entries per warp: cfg2x2, n12288a1): two entries per ticket (cfg2x2 109-110 us against 111 by class).
+        // faster at cfg3 than dealing the very heavy runs one or two entries at a time, and than one entry per ticket everywhere.
+        // Shorter queues: ticket size by the class of the run (dyn_queue_position_zoned), which is what keeps four very heavy
+        // entries from landing on one warp (a uniform 4 is far slower at cfg2x2 and cfg2).
+        // Medium queues (27..72 entries per warp: cfg2x2, n12288a1): two entries per ticket (slightly ahead of by class).
         // The ring words go through st.release / ld.acquire (RING = 2; the volatile formulation times the same, the one in
-        // shared atomics that racecheck accepts costs 13 %: profiles/r2/ab_march_28_ring_handoff.jsonl).
+        // shared atomics that racecheck accepts is slower).
         else if (mq.uniform_ipt4 == 4u && v == 0) launch_lean_t<0, true, false, 4, true, 512, 4, 2>(q, mq, sms * 4u, noise, count, st);
         else if (mq.uniform_ipt4 == 2u && v == 0) launch_lean_t<0, true, false, 4, true, 512, 2, 2>(q, mq, sms * 4u, noise, count, st);
         else launch_lean_t<0, true, false, 4, true, 512, 0, 2>(q, mq, sms * 4u, noise, count, st);
@@ -1389,8 +1387,7 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
                 // the claim for run r + 16 could overwrite the ring slot of run r before it is read)
                 const unsigned sh_max = mq.chunk_shift > 0u ? mq.chunk_shift - 1u : 0u;
                 // queue entries per warp of the launch: one entry per ticket for the very heavy runs, four for the light ones, and
-                // for the heavy runs two on a short queue, four on a longer one (cfg2: 68.3 us with 0:1:2, 69.8 with 0:2:2;
-                // n12288a1 and cfg2x2: 155.9 / 112.0 and 155.1 / 111.7; profiles/r2/ab_march_23_*.jsonl)
+                // for the heavy runs two on a short queue, four on a longer one (measured at cfg2, cfg2x2 and n12288a1)
                 const unsigned per_warp = mq.items / (blocks * 16u);
                 const int dflt[4] = {0, per_warp >= 27u ? 2 : 1, 2, 255};
                 for (int z = 0; z < 4; z++) {
@@ -1477,13 +1474,12 @@ marched:
 
     // largest value a scan entry can hold: the max_range clamp plus 8 sigma of the optional noise
     const double max_scan = map->max_range + 8.0 * (sim->noise_std > 0.0 ? sim->noise_std : 0.0) + 1e-3;
-    // k_tail2 (2 <= A <= 4): cfg3 tail 79 -> 60 us, tick 518 -> 486 us; cfg2x2 28.5 -> 22.6 us once its blocks are small enough to
-    // fill the GPU (profiles/r2/ab_march_16..18_*.jsonl)
+    // k_tail2 (2 <= A <= 4): faster than k_tail at cfg3 and, once its blocks are small enough to fill the GPU, at cfg2x2
     if (sim->num_agents >= 2 && sim->num_agents <= 4 && g_tail2) {
         // two-phase tail: ~64 agents per block (thread per (ego, opponent) pair for the scalar work, warp per ego for the beams);
         // f110_step (no lap logic, no auto-reset) runs the same kernel with the env-level phase switched off
         // up to 64 agents per block, fewer when that would leave SMs without a block (cfg2x2: 4096 envs / 32 = 128 blocks lost
-        // 4 us against 8 envs per block)
+        // against 8 envs per block)
         int epb = g_tail2_forced ? max(1, g_tail2_agents / sim->num_agents) : max(1, min(g_tail2_agents / sim->num_agents, sim->num_envs / (4 * num_sms())));
         AutoResetArgs no_ar;
         no_ar.start_poses = nullptr; no_ar.num_start = 0; no_ar.pose_gap = 0; no_ar.seed = 0; no_ar.tick_host = 0;
@@ -1491,11 +1487,10 @@ marched:
         // big blocks (>= 48 agents) run 256 threads, small ones 128 (measured: 256:64 best at cfg3, 128:12 at cfg2x2)
         int t2 = (g_tail2_threads != F110_TAIL2_THREADS) ? g_tail2_threads : (epb * sim->num_agents >= 48 ? 256 : 128);
         if (!g_tail2_forced && g_tail2_threads == F110_TAIL2_THREADS) {
-            // Whole waves.  With 80 registers an SM holds six 128-thread blocks (three of 256 threads); a grid of 1.37 waves (cfg3:
-            // 607 blocks of 27 envs, 256 threads, on 444 slots) leaves the GPU two-thirds empty for the second half of the kernel:
-            // 59.4 us against 46.8 for 863 blocks of 19 envs on the 888 slots of 128-thread blocks, 46.5 for 443 blocks of 37 envs
-            // at 256 threads (profiles/r2/ab_march_31_tail2_waves.jsonl).  So: 128-thread blocks of up to 47 agents, and as many
-            // envs per block as fill a whole number of waves.
+            // Whole waves.  With 80 registers an SM holds six 128-thread blocks (three of 256 threads); a grid of about 1.4 waves
+            // leaves the GPU two-thirds empty for the second half of the kernel, and grids of whole waves measured about a quarter
+            // faster.  So: 128-thread blocks of up to 47 agents, and as many envs per block as fill a whole number of waves
+            // (the wave size comes from the occupancy query and the SM count, not from a fixed device).
             static int per_sm = 0;                          // resident 128-thread blocks per SM
             if (per_sm == 0) {
                 const size_t sm0 = (size_t)(47 / sim->num_agents) * sim->num_agents * (sim->num_agents - 1) * sizeof(TailTask);

@@ -71,8 +71,8 @@ __device__ __noinline__ double escape_load(const double *__restrict__ cells, uns
 // Work queue of the persistent march kernel (exactness never depends on it).
 // Lookups per beam are heavy-tailed (p50 5, p99 32, max ~300 under the benchmark policy) and a long
 // beam is a serial dependent chain (~150 ns per lookup).  With one block per tile of beams the grid's
-// makespan was 60 us of throughput phase plus a 37 us tail of a few late-dispatched tiles holding a
-// 250-lookup beam, and the block dispatcher could not keep all slots filled (profiles/r1/).  So:
+// makespan was a throughput phase plus a long tail of a few late-dispatched tiles holding a
+// 250-lookup beam, and the block dispatcher could not keep all slots filled.  So:
 //   * work items are 32 consecutive beams of one agent (one warp); every item records its maximum lookup
 //     count, which changes little from tick to tick (>= 99 % of the items with a >= 100-lookup beam had
 //     a >= 24-lookup beam one tick earlier);
@@ -119,8 +119,8 @@ __device__ __forceinline__ void march_beam(const MarchK &p, unsigned a, int i, d
     // + index) on every lookup, 4 address instructions instead of one IMAD.WIDE (loop 27 -> 23 instructions).
     // Things tried on the remaining 4 parameter re-loads per iteration (ptxas rematerialises them; it sees through
     // moves and uniform shuffles): pinning them in registers via volatile shared-memory reads gives a 20-instruction
-    // loop but needs 40 registers = 48 warps/SM: 83 us vs 77 us (occupancy beats instruction count here); unrolling
-    // the loop by two (21.5 instructions per lookup): 78.5 us vs 76.9 us.
+    // loop but needs 40 registers = 48 warps/SM, and was slower (occupancy beats instruction count here); unrolling
+    // the loop by two (21.5 instructions per lookup) was slower too.
     const double *table = (CELLS ? p.cells : p.dt) + lo;
     asm volatile("" : "+l"(table));
     const int ti = beam_theta_index(ti0, i, p.inc, p.theta_dis_f, p.ti_guard);
@@ -244,9 +244,9 @@ __global__ void __launch_bounds__(PT, 4) k_march_persistent(const MarchK p, cons
         if (lane == 0) k = atomicAdd(&s_next, 1u);
         k = __shfl_sync(0xffffffffu, k, 0);
         // items < 2^32 / 4 (host-checked): no overflow.  Consecutive entries of a class list are neighbouring
-        // slices of one agent, so dealing them in runs of 8 lets the warps of a block share L1 lines (march 80.5 ->
-        // 77.2 us at cfg2; runs of 4 / 16: 80.6 / 79.5 us; also giving the co-resident blocks of an SM neighbouring
-        // runs concentrates the heavy items on few SMs: 86.7 us).
+        // slices of one agent, so dealing them in runs of 8 lets the warps of a block share L1 lines (faster at cfg2
+        // than runs of 4 or 16; also giving the co-resident blocks of an SM neighbouring runs concentrates the heavy
+        // items on few SMs and is slower still).
         const unsigned q = ((((k >> mq.chunk_shift) * gridDim.x + blockIdx.x) << mq.chunk_shift)) +
                            (k & ((1u << mq.chunk_shift) - 1u));
         if (q >= total) break;

@@ -1,8 +1,8 @@
 // march_lean.cuh — k_march_lean: the production ray-march kernel of f110_step / f110_tick (round 2).
 //
 // Same results as march.cuh's k_march_persistent (bit-identical ranges, same DT lookups), same persistent
-// longest-first work queue; what changed is the instruction count.  The round-1 SASS (profiles/r2/README.md) spent
-// ~170 of its ~365 warp-instructions per 32-beam work item OUTSIDE the sphere-tracing loop and carried four
+// longest-first work queue; what changed is the instruction count.  The round-1 SASS spent
+// about half of its warp-instructions per 32-beam work item OUTSIDE the sphere-tracing loop and carried four
 // kernel-parameter reloads inside it.  Here:
 //   * everything that is constant for an agent is computed once per agent by k_dynamics into a 64-byte record
 //     (scan position already in cell units, first lookup, LUT index of beam 0 as Q16.48 fixed point, the iTTC
@@ -106,14 +106,14 @@ __device__ __noinline__ double redo_beam_cells(const double *__restrict__ table,
 // TABLE: 0 = fp64 table in global memory, 1 = u8 rank codes in global memory + fp64 LUT in shared memory
 // DYN: the first mq.static_runs runs (of 2^chunk_shift consecutive queue entries) of every block are dealt statically,
 // round-robin, as before; the REST of the queue is handed out dynamically from one global counter (mq.claim).  Static
-// dealing gives every block the same number of items but not the same amount of work: ncu showed the SMs busy for only
-// 83 % of the kernel's duration at cfg2 and 95 % at cfg3 (profiles/r2).  Claims are prefetched: the warp that draws the first
+// dealing gives every block the same number of items but not the same amount of work: some SMs finish early and idle
+// until the last block ends.  Claims are prefetched: the warp that draws the first
 // ticket of local run r claims the run for r + mq.dyn_ahead and publishes it in a shared-memory ring, so a ticket only reads
-// two shared words; the global order of the queue (longest first) is kept.  Two lessons from the A/B (profiles/r2/README.md):
+// two shared words; the global order of the queue (longest first) is kept.  Two lessons from the A/B measurements:
 //   * the ring logic must stay OUT OF LINE (dyn_queue_position): inlined it wrecks the register allocation of the whole item
-//     path (55.4 M instead of 43.6 M warp-instructions per launch) and every dynamic flavour loses by 15-25 %;
-//   * half static / half dynamic is the optimum (cfg3 march 443 -> 407 us with 4 x 512 threads per SM, better than the static
-//     2 x 1024 shape's 419; 85 % static loses, 10-30 % is 1-2 % behind): the static half keeps the head of the queue -- the
+//     path (a quarter more warp-instructions per launch) and every dynamic flavour loses;
+//   * half static / half dynamic was the measured optimum (with 4 x 512 threads per SM, also ahead of the static 2 x 1024
+//     shape; a mostly static or a mostly dynamic split is behind): the static half keeps the head of the queue -- the
 //     heavy items -- free of claim latency, the dynamic half evens out the blocks.
 #define F110_DYN_RING 16u
 // common tail of the two ticket -> queue position functions: (local run r, first entry idx of the ticket inside the run,
@@ -181,8 +181,8 @@ __device__ __noinline__ unsigned dyn_queue_position(unsigned k, bool elected, un
 }
 // Ticket size by the class of the run (k_march_lean<IPT = 0>).  The queue holds the very heavy entries first, then the heavy,
 // then the light ones: a ticket of four consecutive VERY HEAVY entries puts four of the longest marches of the launch on one
-// warp, one after the other -- a constant ~30 us on the critical path at every batch size (ab_march_21/22: 4 entries per ticket
-// won 10 % at cfg3 and lost 25 % at cfg2x2) -- while for the light entries the pop and this call are a large part of the work.
+// warp, one after the other -- a constant addition to the critical path at every batch size (4 entries per ticket won at
+// cfg3 and lost at cfg2x2) -- while for the light entries the pop and this call are a large part of the work.
 // zone[] (shared memory, written by thread 0 before the first pop): ticket bounds T1 <= T2 <= T3 of the block's static runs
 // that start in the very heavy / heavy / light part of the queue, the run counts rA, rAB behind them, and the four shifts
 // (very heavy | heavy << 8 | light << 16 | dynamic tail << 24).
@@ -203,10 +203,10 @@ __device__ __noinline__ unsigned dyn_queue_position_zoned(unsigned k, bool elect
 // the cluster's rank-0 CTA, popped through distributed shared memory: mapa + atom.shared::cluster).  The queue is then dealt
 // statically to the CLUSTERS and handed out dynamically inside each: a pool of CL x PT/32 warps on several SMs of one GPC
 // instead of PT/32 warps on one SM, which evens out the finishing times without the global atomics that made the fully
-// dynamic queue lose (profiles/r2/README.md).
+// dynamic queue lose.
 // IPT: queue entries per ticket (1, 2 or 4; 0 = by the class of the run, mq.ipt_shifts, dynamic queue only).  With 2, a warp that
 // pops the block's counter marches two consecutive entries of its run before it pops again: the pop, the queue arithmetic and
-// the dynamic-queue call are paid once per 64 beams (profiles/r2/ab_march_19..23_*.jsonl).
+// the dynamic-queue call are paid once per 64 beams.
 template <int TABLE, bool NOISE, bool COUNT, bool CELLS, bool LAYERED, int PT, int MINB, bool DYN = false, int CL = 1, int IPT = 1, int RING = 0>
 __global__ void __launch_bounds__(PT, MINB) k_march_lean(const LeanK p, const MarchQueue mq) {
     __shared__ unsigned s_next;

@@ -2,7 +2,7 @@
 // each agent's scan pose is staged into SHARED memory by TMA (cp.async.bulk.tensor.2d, mbarrier completion) and the
 // agent's beams march through it on chip; lookups that leave the tile fall back to the global table.
 //
-// Why: k_march_lean is latency bound (profiles/r2: long-scoreboard 11 warps per issue, L1 hit rate 53 %, 21.8 cycles
+// Why: k_march_lean is latency bound (long-scoreboard 11 warps per issue, L1 hit rate 53 %, 21.8 cycles
 // per instruction per warp): every sphere-tracing step is a dependent, divergent 8-byte gather that misses L1 half of
 // the time because the ~10 agents an SM works on at once have a 40-130 KB footprint each in the 8-byte table.  The
 // tile holds the near field (where the lookups are dense) as 1-byte rank codes: TILE x TILE cells = 16 KB, decoded

@@ -116,7 +116,7 @@ def device_edt(bitmap, resolution, device):
 
 
 def load_map_device_edt(map_path, map_ext, device):
-    """Same map, with the distance transform done on the device (~1 ms instead of ~1.5 s for 1600x1600)."""
+    """Same map, with the distance transform done on the device (exact, same table as scipy's)."""
     img, resolution, origin = load_bitmap(map_path, map_ext)
     dt = device_edt(img, resolution, device)
     return HostMap(dt.cpu().numpy(), resolution, origin)

@@ -1,5 +1,5 @@
 /*
- * f110_b200.h — C ABI of the B200-native batched F1TENTH hot path (libf110_b200.so).
+ * f110_b200.h — C ABI of the batched F1TENTH hot path for the H100 (libf110_b200.so).
  *
  * The reference (f1tenth/f1tenth_gym) is pure Python + numba and has no FFI of its own; its
  * boundary for this path is the Python surface  F110Env -> Simulator -> @njit kernels.  Each entry

@@ -12,7 +12,7 @@ MAPS = os.path.join(ROOT, 'f1tenth_gym_b200', 'maps')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: test needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: test needs a CUDA device (run on an H100)')
 
 
 @pytest.fixture(scope='session')

@@ -96,7 +96,7 @@ def test_library_exports_every_declared_symbol():
 def test_march_kernel_resource_budget():
     """The production ray-march kernels must keep the register and stack budget the measurements were taken with: 32 registers
     (64 warps per SM) and at most 24 bytes of stack per thread.  A same-results build whose caller-side spills grew to 56 bytes of
-    stack was 13 % slower (profiles/r2/README.md, "What ptxas does to this kernel"): this is the check to run after any edit to
+    stack was measurably slower (DESIGN.md 3.2, codegen caveat): this is the check to run after any edit to
     csrc/march_lean.cuh, before spending GPU time."""
     import shutil
     from f1tenth_gym_b200 import _native as nat
@@ -119,8 +119,8 @@ def test_march_kernel_resource_budget():
         assert stack <= 24, (name, stack)
 
 
-def test_sass_carries_the_sm100a_paths():
-    """The built library is sm_100a code and contains what DESIGN.md says it does: the TMA tile load of the north_star march variant
+def test_sass_carries_the_sm90a_paths():
+    """The built library is sm_90a code and contains what DESIGN.md says it does: the TMA tile load of the north_star march variant
     (UTMALDG with mbarrier SYNCS), the elect.sync queue pop (ELECT) and the programmatic-dependent-launch hooks (ACQBULK / PREEXIT)."""
     import shutil
     from f1tenth_gym_b200 import _native as nat
@@ -130,7 +130,7 @@ def test_sass_carries_the_sm100a_paths():
     nat.lib()
     lib_path = os.path.join(os.path.dirname(os.path.abspath(nat.__file__)), 'libf110_b200.so')
     elf = subprocess.run([tool, '-lelf', lib_path], capture_output=True, text=True).stdout
-    assert 'sm_100a' in elf, elf
+    assert 'sm_90a' in elf and 'sm_100' not in elf, elf
     sass = subprocess.run([tool, '-sass', lib_path], capture_output=True, text=True).stdout
     for mnemonic in ('UTMALDG', 'SYNCS', 'ELECT', 'ACQBULK', 'PREEXIT', 'DADD.RM'):
         assert mnemonic in sass, mnemonic

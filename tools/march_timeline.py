@@ -45,8 +45,9 @@ dur = end - start
 print('block duration us: mean %.2f p50 %.2f p90 %.2f p99 %.2f max %.2f' % (dur.mean(), *np.percentile(dur, [50, 90, 99]), dur.max()))
 print('steps(max of warp0): mean %.1f p99 %d max %d' % (tr[:, 3].mean(), np.percentile(tr[:, 3], 99), tr[:, 3].max()))
 print('last block START at %.1f us' % start.max())
-sm_end = np.zeros(148); sm_busy = np.zeros(148)
-for s in range(148):
+nsm = torch.cuda.get_device_properties(0).multi_processor_count
+sm_end = np.zeros(nsm); sm_busy = np.zeros(nsm)
+for s in range(nsm):
     m = tr[:, 0] == s
     if m.any():
         sm_end[s] = end[m].max()
