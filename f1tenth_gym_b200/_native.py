@@ -105,6 +105,7 @@ DEBUG_SIGNATURES = {
     'f110_debug_set_tail': (None, [C.c_int]),
     'f110_debug_set_tail2': (None, [C.c_int, C.c_int]),
     'f110_debug_set_tile_counter': (None, [C.c_void_p]),
+    'f110_debug_last_launch': (C.c_char_p, []),
 }
 
 _LIB = None

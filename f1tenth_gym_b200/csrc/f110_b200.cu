@@ -962,6 +962,10 @@ static int check_beams(const f110_beams *b) {
 
 static unsigned long long *g_trace = nullptr;
 static unsigned long long *g_tile_counter = nullptr;   // debug only: lookups served from the shared-memory tile   // debug only: per-block timeline buffer (f110_debug_set_trace)
+// debug record of the kernels the last step_impl of this thread launched (f110_debug_last_launch): host-side text only; the
+// launch helpers fill the march part, step_impl adds the queue figures and the tail
+static thread_local char g_launch_march[192] = "";
+static thread_local char g_launch_rec[384] = "";
 
 static int num_sms() {
     static int n = 0;
@@ -997,6 +1001,8 @@ static int launch_raymarch(const MapView &mv, const BeamView &bv, const MarchArg
     const int threads = 256;
     const long long blocks = (g.total + threads - 1) / threads;
     if (blocks <= 0 || blocks > 0x7fffffffll) return F110_ERR_INVALID;
+    snprintf(g_launch_march, sizeof(g_launch_march), "march=literal FAST=%d NOISE=%d COUNT=%d PT=%d grid=%lld", fast ? 1 : 0,
+             g.noise_std > 0.0 ? 1 : 0, g.lookup_counter ? 1 : 0, threads, blocks);
     if (fast) {
         if (standalone) k_raymarch<true, true><<<(unsigned)blocks, threads, 0, st>>>(mv, bv, g);
         else k_raymarch<true, false><<<(unsigned)blocks, threads, 0, st>>>(mv, bv, g);
@@ -1011,6 +1017,8 @@ static int launch_raymarch(const MapView &mv, const BeamView &bv, const MarchArg
 template <int PT, int SUB, bool CELLS>
 static void launch_persistent(const MarchK &k, const MarchQueue &mq, unsigned blocks, bool coded, bool noise, bool count,
                               cudaStream_t st) {
+    snprintf(g_launch_march, sizeof(g_launch_march), "march=persistent CELLS=%d CODED=%d NOISE=%d COUNT=%d SUB=%d PT=%d grid=%u",
+             CELLS ? 1 : 0, coded ? 1 : 0, noise ? 1 : 0, count ? 1 : 0, SUB, PT, blocks);
     if (k.trace) {
         if (coded && CELLS) k_march_persistent<CELLS, false, false, true, PT, SUB, CELLS><<<blocks, PT, 0, st>>>(k, mq);
         else k_march_persistent<false, false, false, true, PT, SUB, CELLS><<<blocks, PT, 0, st>>>(k, mq);
@@ -1073,6 +1081,9 @@ static bool clusters_fit(K kernel, unsigned blocks, unsigned threads, unsigned c
 template <int TABLE, bool CELLS, bool LAYERED, int MINB, bool DYN = false, int PT = 512, int IPT = 1, int RING = 0>
 static void launch_lean_t(const LeanK &q, const MarchQueue &mq, unsigned blocks, bool noise, bool count, cudaStream_t st) {
     const bool pdl = g_pdl_this_step;
+    snprintf(g_launch_march, sizeof(g_launch_march),
+             "march=lean TABLE=%d CELLS=%d LAYERED=%d DYN=%d IPT=%d RING=%d PT=%d MINB=%d NOISE=%d COUNT=%d grid=%u", TABLE,
+             CELLS ? 1 : 0, LAYERED ? 1 : 0, DYN ? 1 : 0, IPT, RING, PT, MINB, noise ? 1 : 0, count ? 1 : 0, blocks);
     if (count) launch_k(k_march_lean<TABLE, false, true, CELLS, LAYERED, PT, MINB, DYN, 1, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
     else if (noise) launch_k(k_march_lean<TABLE, true, false, CELLS, LAYERED, PT, MINB, DYN, 1, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
     else launch_k(k_march_lean<TABLE, false, false, CELLS, LAYERED, PT, MINB, DYN, 1, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
@@ -1091,7 +1102,7 @@ static void launch_lean(const LeanK &q, const MarchQueue &mq, unsigned sms, bool
                        if ((ok = clusters_fit(k, sms * 4u, 512, 4))) launch_cluster(k, dim3(sms * 4u), dim3(512), 4, st, q, mq); }
         if (v == 65) { auto k = k_march_lean<0, false, false, true, false, 512, 4, false, 8>;
                        if ((ok = clusters_fit(k, sms * 4u / 8u * 8u, 512, 8))) launch_cluster(k, dim3(sms * 4u / 8u * 8u), dim3(512), 8, st, q, mq); }
-        if (ok) return;
+        if (ok) { snprintf(g_launch_march, sizeof(g_launch_march), "march=lean-cluster variant=%d", v); return; }
         if (getenv("F110_DEBUG")) fprintf(stderr, "f110: cluster variant %d does not fit, using the default launch\n", v);
     }
     // Block shape at the same 64 warps/SM.  Two 1024-thread blocks per SM (32 warps share a ticket counter, the queue is dealt
@@ -1183,6 +1194,8 @@ static int launch_tile_t(const TileK &t, const f110_map *map, unsigned sms, bool
     const size_t smem = sizeof(TileSmem<TILE, NSLOT>);
     constexpr int PT = 512;
     constexpr int MINB = 4;
+    snprintf(g_launch_march, sizeof(g_launch_march), "march=tile TILE=%d NSLOT=%d NOISE=%d COUNT=%d PT=%d MINB=%d grid=%u", TILE, NSLOT,
+             noise ? 1 : 0, count ? 1 : 0, PT, MINB, sms * MINB);
     if (count) {
         CUDA_TRY(cudaFuncSetAttribute(k_march_tile<false, true, TILE, NSLOT, PT, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         k_march_tile<false, true, TILE, NSLOT, PT, MINB><<<sms * MINB, PT, smem, st>>>(t, tm);
@@ -1202,6 +1215,8 @@ static int launch_tile(const TileK &t, const f110_map *map, int tile_sz, unsigne
 
 template <int MINB, bool CELLS>
 static void launch_march(const MarchK &k, dim3 grid, bool coded, bool noise, bool count, cudaStream_t st) {
+    snprintf(g_launch_march, sizeof(g_launch_march), "march=block-per-tile CELLS=%d CODED=%d NOISE=%d COUNT=%d MINB=%d grid=%ux%u",
+             CELLS ? 1 : 0, coded ? 1 : 0, noise ? 1 : 0, count ? 1 : 0, MINB, grid.x, grid.y);
     if (coded && CELLS) {
         if (count) k_march<CELLS, false, true, MINB, CELLS><<<grid, 64, 0, st>>>(k);
         else if (noise) k_march<CELLS, true, false, MINB, CELLS><<<grid, 64, 0, st>>>(k);
@@ -1251,6 +1266,9 @@ void f110_debug_set_tail(int minb) {      // -1: k_tail always; -2 or a register
 }
 void f110_debug_set_tile_counter(unsigned long long *buf) { g_tile_counter = buf; }
 void f110_debug_set_chunk(int chunk_shift) { g_chunk = (chunk_shift < 0 || chunk_shift > 6) ? 3 : chunk_shift; }
+/* test aid (not in the public header): `key=value` record of the kernels the last step / tick of the calling thread launched
+ * (march kernel family and template choices, queue figures, tail kernel and shape); empty before the first one */
+const char *f110_debug_last_launch(void) { return g_launch_rec; }
 
 const char *f110_status_string(int status) {
     switch (status) {
@@ -1287,6 +1305,10 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
 
     if (ev) CUDA_TRY(cudaEventRecord(ev[0], st));
     g_pdl_this_step = (ev == nullptr);
+    g_launch_march[0] = '\0';
+    g_launch_rec[0] = '\0';
+    unsigned rec_per_warp = 0u, rec_static_runs = 0u;          // (debug record only)
+    char rec_tail[96] = "";
     const int variant = rm_variant();
     // work-item width: march_ipa = ceil(B/32) -> one 32-beam slice per item, ceil(B/64) -> two
     const int item_sub = (sim->march_ipa == (beams->num_beams + 31) / 32) ? 1
@@ -1389,6 +1411,8 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
                 // queue entries per warp of the launch: one entry per ticket for the very heavy runs, four for the light ones, and
                 // for the heavy runs two on a short queue, four on a longer one (measured at cfg2, cfg2x2 and n12288a1)
                 const unsigned per_warp = mq.items / (blocks * 16u);
+                rec_per_warp = per_warp;
+                rec_static_runs = mq.static_runs;
                 const int dflt[4] = {0, per_warp >= 27u ? 2 : 1, 2, 255};
                 for (int z = 0; z < 4; z++) {
                     const int want = g_ipt[z] < 0 ? dflt[z] : g_ipt[z];
@@ -1505,6 +1529,8 @@ marched:
             }
         }
         const size_t smem = (size_t)epb * sim->num_agents * (sim->num_agents - 1) * sizeof(TailTask);
+        snprintf(rec_tail, sizeof(rec_tail), "tail=k_tail2 epb=%d threads=%d tail_grid=%d smem=%zu", epb, t2,
+                 (sim->num_envs + epb - 1) / epb, smem);
         launch_k(k_tail2, dim3((sim->num_envs + epb - 1) / epb), dim3(t2), smem, st, g_pdl_this_step && lean, *sim, bv,
                  fused ? (int)tail->env_level : 0, fused ? tail->ar : no_ar, max_scan, epb);
         LAUNCH_CHECK("k_tail2");
@@ -1514,6 +1540,8 @@ marched:
         const int threads = 32 * sim->num_agents * epb;
         const dim3 tgrid((sim->num_envs + epb - 1) / epb);
         const bool tpdl = g_pdl_this_step && lean;
+        snprintf(rec_tail, sizeof(rec_tail), "tail=k_tail<%d,%d> epb=%d threads=%d tail_grid=%u", threads <= 128 ? 128 : 1024,
+                 threads > 128 ? 1 : (g_tail_minb == 4 || g_tail_minb == 5) ? g_tail_minb : 8, epb, threads, tgrid.x);
         // register budget of the 128-thread flavour (A <= 4): 4 blocks/SM = 128 registers (no spills), 5 = 96, 8 = 64
         if (threads <= 128 && g_tail_minb == 4)
             launch_k(k_tail<128, 4>, tgrid, dim3(threads), 0, st, tpdl, *sim, bv, (int)tail->env_level, tail->ar, max_scan, epb);
@@ -1526,6 +1554,8 @@ marched:
                      (int)tail->env_level, tail->ar, max_scan, epb);
         LAUNCH_CHECK("k_tail");
     } else {
+        snprintf(rec_tail, sizeof(rec_tail), "tail=k_finalize%s epb=0 threads=128 tail_grid=%d",
+                 (tail && tail->fused) ? "+separate" : "", (NA * 32 + 127) / 128);
         launch_k(k_finalize, dim3((NA * 32 + 127) / 128), dim3(128), 0, st, g_pdl_this_step && lean, *sim, bv, max_scan);
         LAUNCH_CHECK("k_finalize");
         if (tail && tail->fused) {     // more than 32 agents per env: same semantics with separate launches
@@ -1533,6 +1563,8 @@ marched:
             if (tail->ar.start_poses) { k_autoreset<<<(sim->num_envs + 127) / 128, 128, 0, st>>>(*sim, tail->ar); LAUNCH_CHECK("k_autoreset"); }
         }
     }
+    snprintf(g_launch_rec, sizeof(g_launch_rec), "%s static_runs=%u per_warp=%u %s", g_launch_march, rec_static_runs, rec_per_warp,
+             rec_tail);
     if (ev) CUDA_TRY(cudaEventRecord(ev[3], st));
     return F110_OK;
 }

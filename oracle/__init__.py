@@ -88,6 +88,11 @@ def lib():
         L.orc_rollout.restype = C.c_int64
         L.orc_rollout.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int, _dp, C.c_int, C.c_int,
                                   C.c_uint64, C.c_int, C.POINTER(C.c_int64)]
+        L.orc_sim_scans_pre.restype = _dp
+        L.orc_sim_scans_pre.argtypes = [C.c_void_p]
+        L.orc_env_restart.argtypes = [C.c_void_p, _dp]
+        L.orc_step_batch.argtypes = [C.POINTER(C.c_void_p), C.c_int, _dp, _dp, C.c_int, C.c_int]
+        L.orc_gather.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int, _dp]
         L.orc_pure_pursuit.argtypes = [_dp, _dp, _dp, C.c_int] + [C.c_double] * 7 + [_dp]
         L.orc_num_cores.restype = C.c_int
         _LIB = L
@@ -276,6 +281,7 @@ class OracleSim(object):
         self.in_collision = np.ctypeslib.as_array(L.orc_sim_in_collision(h), (A,))
         self.steer_cnt = np.ctypeslib.as_array(L.orc_sim_steer_cnt(h), (A,))
         self.steer_buf = np.ctypeslib.as_array(L.orc_sim_steer_buf(h), (A, 2))
+        self.scans_pre = np.ctypeslib.as_array(L.orc_sim_scans_pre(h), (A, B))
 
     def __del__(self):
         try:
@@ -308,6 +314,48 @@ class OracleSim(object):
 
     def env_post_step(self):
         return bool(lib().orc_env_post_step(self._h))
+
+    def env_restart(self, poses):
+        """The device auto-reset of this env (f110_autoreset): Simulator.reset + env counters and start frame, no
+        zero-action step; `done` and the collision observation of the ending tick are kept."""
+        poses = _f64(poses)
+        assert poses.shape == (self.num_agents, 3)
+        lib().orc_env_restart(self._h, _p(poses))
+
+
+_FIELDS = {'state': 0, 'scans': 1, 'scans_pre': 2, 'collisions': 3, 'collision_idx': 4, 'in_collision': 5,
+           'lap_times': 6, 'lap_counts': 7, 'toggle_list': 8, 'done': 9, 'current_time': 10, 'nlook': 11}
+
+
+def _handles(sims):
+    return (C.c_void_p * len(sims))(*[s._h for s in sims])
+
+
+def step_batch(sims, actions, noise=None, env_level=False, num_threads=0):
+    """One step of every OracleSim in `sims` (same num_agents / num_beams), spread over the host cores.
+    actions (n, A, 2); noise (n, A, B) additive scan noise or None; env_level: also the F110Env lap logic and done
+    (read back with gather(sims, 'done'))."""
+    n = len(sims)
+    A, B = sims[0].num_agents, sims[0].num_beams
+    a = _f64(actions)
+    assert a.shape == (n, A, 2)
+    nz = None
+    if noise is not None:
+        nz = _f64(noise)
+        assert nz.shape == (n, A, B)
+    lib().orc_step_batch(_handles(sims), n, _p(a), None if nz is None else _p(nz), 1 if env_level else 0, num_threads)
+
+
+def gather(sims, field):
+    """One field of every sim as an array: (n, A, 7) state, (n, A, B) scans / scans_pre, (n,) done / current_time /
+    nlook, (n, A) otherwise."""
+    n = len(sims)
+    A, B = sims[0].num_agents, sims[0].num_beams
+    shape = {'state': (n, A, 7), 'scans': (n, A, B), 'scans_pre': (n, A, B), 'done': (n,), 'current_time': (n,),
+             'nlook': (n,)}.get(field, (n, A))
+    out = np.empty(shape)
+    lib().orc_gather(_handles(sims), n, _FIELDS[field], _p(out))
+    return out
 
 
 def rollout(sims, ticks, start_poses, pose_gap=23, seed=12345, num_threads=0):

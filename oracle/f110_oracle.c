@@ -397,6 +397,10 @@ typedef struct {
     double *start_xs, *start_ys, *start_thetas;   /* [A] */
     double start_rot[4];
     int64_t nlook;       /* DT lookups performed so far */
+    /* batch driver (orc_step_batch) */
+    const double *noise; /* [A][B] additive scan noise of the current step, or NULL */
+    double *scans_pre;   /* [A][B] each agent's scan before the opponent ray-cast (after noise) */
+    int32_t done;        /* result of the last orc_env_post_step */
 } orc_sim_t;
 
 orc_sim_t *orc_sim_create(int num_agents, int num_beams, int integrator, double time_step, double fov,
@@ -420,6 +424,7 @@ orc_sim_t *orc_sim_create(int num_agents, int num_beams, int integrator, double 
     s->collision_idx = (double *)calloc(A, sizeof(double));
     s->agent_poses = (double *)calloc(A * 3, sizeof(double));
     s->scans = (double *)calloc((size_t)A * B, sizeof(double));
+    s->scans_pre = (double *)calloc((size_t)A * B, sizeof(double));
     s->lap_times = (double *)calloc(A, sizeof(double));
     s->lap_counts = (double *)calloc(A, sizeof(double));
     s->toggle_list = (double *)calloc(A, sizeof(double));
@@ -435,7 +440,7 @@ orc_sim_t *orc_sim_create(int num_agents, int num_beams, int integrator, double 
 void orc_sim_destroy(orc_sim_t *s) {
     if (!s) return;
     free(s->params); free(s->state); free(s->steer_buf); free(s->steer_cnt); free(s->in_collision);
-    free(s->collisions); free(s->collision_idx); free(s->agent_poses); free(s->scans);
+    free(s->collisions); free(s->collision_idx); free(s->agent_poses); free(s->scans); free(s->scans_pre);
     free(s->lap_times); free(s->lap_counts); free(s->toggle_list); free(s->near_starts);
     free(s->start_xs); free(s->start_ys); free(s->start_thetas);
     free(s);
@@ -444,6 +449,7 @@ void orc_sim_destroy(orc_sim_t *s) {
 /* accessors for ctypes */
 double *orc_sim_state(orc_sim_t *s) { return s->state; }
 double *orc_sim_scans(orc_sim_t *s) { return s->scans; }
+double *orc_sim_scans_pre(orc_sim_t *s) { return s->scans_pre; }
 double *orc_sim_collisions(orc_sim_t *s) { return s->collisions; }
 double *orc_sim_collision_idx(orc_sim_t *s) { return s->collision_idx; }
 double *orc_sim_lap_times(orc_sim_t *s) { return s->lap_times; }
@@ -507,8 +513,13 @@ static void update_pose(orc_sim_t *s, int i, double raw_steer, double vel) {
     else if (st[4] < 0) st[4] = st[4] + 2 * M_PI;
     /* :406-410 scan pose */
     double scan_pose[3] = { st[0] + s->lidar_dist * cos(st[4]), st[1] + s->lidar_dist * sin(st[4]), st[4] };
-    orc_get_scan(s->map, scan_pose, s->num_beams, s->fov, s->theta_index_increment,
-                 s->scans + (size_t)i * s->num_beams, &s->nlook);
+    double *scan = s->scans + (size_t)i * s->num_beams;
+    orc_get_scan(s->map, scan_pose, s->num_beams, s->fov, s->theta_index_increment, scan, &s->nlook);
+    /* laser_models.py:450-452: the noise is part of the scan that check_ttc and the opponent ray-cast see */
+    if (s->noise) {
+        const double *nz = s->noise + (size_t)i * s->num_beams;
+        for (int b = 0; b < s->num_beams; b++) scan[b] = scan[b] + nz[b];
+    }
 }
 
 /* base_classes.py:553-612 Simulator.step.  control_inputs [A][2] = (steer, speed). */
@@ -535,6 +546,7 @@ void orc_sim_step(orc_sim_t *s, const double *control_inputs) {
         int hit = orc_check_ttc(scan, B, st[3], s->cosines, s->side_distances, s->ttc_thresh);
         if (hit) { st[3] = 0.; st[4] = 0.; st[5] = 0.; st[6] = 0.; }
         s->in_collision[i] = hit;
+        memcpy(s->scans_pre + (size_t)i * B, scan, sizeof(double) * B);
         /* ray_cast_agents :206-227 (opponent vertices use this agent's own length/width) */
         const double *p = s->params + ORC_NPARAM * i;
         double pose[3] = { st[0], st[1], st[4] };
@@ -589,6 +601,86 @@ int orc_env_reset(orc_sim_t *s, const double *poses) {
     orc_sim_step(s, zero);
     free(zero);
     return orc_env_post_step(s);
+}
+
+/* The device auto-reset (include/f110_b200.h f110_autoreset) applied to one env: Simulator.reset to `poses`, the env
+ * counters and start frame of F110Env.reset (f110_env.py:319-331).  Unlike orc_env_reset there is no zero-action step,
+ * and `done` and the collision observation of the tick that ended the episode stay as they are. */
+void orc_env_restart(orc_sim_t *s, const double *poses /* [A][3] */) {
+    int A = s->num_agents;
+    s->current_time = 0.0;
+    for (int i = 0; i < A; i++) {
+        s->near_starts[i] = 1; s->toggle_list[i] = 0.;
+        s->start_xs[i] = poses[3 * i]; s->start_ys[i] = poses[3 * i + 1]; s->start_thetas[i] = poses[3 * i + 2];
+    }
+    double th = -s->start_thetas[s->ego_idx];
+    s->start_rot[0] = cos(th); s->start_rot[1] = -sin(th);
+    s->start_rot[2] = sin(th); s->start_rot[3] = cos(th);
+    orc_sim_reset(s, poses);
+}
+
+/* ------------------------------------------------------------------ batched step (large-batch parity tests)
+ * Steps n independent sims once each: sims[e] with actions + e*A*2 and, when `noise` is not NULL, the additive scan noise
+ * noise + e*A*B; env_level != 0 also runs orc_env_post_step (result in `done`).  pthreads over envs, like orc_rollout. */
+typedef struct {
+    orc_sim_t **sims; int e0, e1, env_level; const double *actions, *noise;
+} batch_job_t;
+
+static void *batch_worker(void *arg) {
+    batch_job_t *jb = (batch_job_t *)arg;
+    for (int e = jb->e0; e < jb->e1; e++) {
+        orc_sim_t *s = jb->sims[e];
+        const size_t A = (size_t)s->num_agents, B = (size_t)s->num_beams;
+        s->noise = jb->noise ? jb->noise + (size_t)e * A * B : NULL;
+        orc_sim_step(s, jb->actions + (size_t)e * A * 2);
+        s->noise = NULL;
+        if (jb->env_level) s->done = orc_env_post_step(s);
+    }
+    return NULL;
+}
+
+/* nthreads <= 0 -> one thread per online core.  Every sim of one call must have the same num_agents / num_beams. */
+void orc_step_batch(orc_sim_t **sims, int n, const double *actions /* [n][A][2] */, const double *noise /* [n][A][B] or NULL */,
+                    int env_level, int nthreads) {
+    if (n <= 0) return;
+    if (nthreads <= 0) nthreads = (int)sysconf(_SC_NPROCESSORS_ONLN);
+    if (nthreads > n) nthreads = n;
+    if (nthreads < 1) nthreads = 1;
+    pthread_t *th = (pthread_t *)malloc(sizeof(pthread_t) * nthreads);
+    batch_job_t *jobs = (batch_job_t *)calloc(nthreads, sizeof(batch_job_t));
+    for (int t = 0; t < nthreads; t++) {
+        jobs[t].sims = sims; jobs[t].env_level = env_level; jobs[t].actions = actions; jobs[t].noise = noise;
+        jobs[t].e0 = (int)((int64_t)n * t / nthreads);
+        jobs[t].e1 = (int)((int64_t)n * (t + 1) / nthreads);
+        pthread_create(&th[t], NULL, batch_worker, &jobs[t]);
+    }
+    for (int t = 0; t < nthreads; t++) pthread_join(th[t], NULL);
+    free(th); free(jobs);
+}
+
+/* Copies one field of n sims into a contiguous array (per sim: A values, A*7 for the state, A*B for the scans, one for
+ * done and current_time), so that a test can compare a whole batch with one array operation. */
+enum { ORC_F_STATE = 0, ORC_F_SCANS, ORC_F_SCANS_PRE, ORC_F_COLLISIONS, ORC_F_COLLISION_IDX, ORC_F_IN_COLLISION,
+       ORC_F_LAP_TIMES, ORC_F_LAP_COUNTS, ORC_F_TOGGLE_LIST, ORC_F_DONE, ORC_F_CURRENT_TIME, ORC_F_NLOOK };
+void orc_gather(orc_sim_t **sims, int n, int field, double *out) {
+    for (int e = 0; e < n; e++) {
+        orc_sim_t *s = sims[e];
+        const size_t A = (size_t)s->num_agents, B = (size_t)s->num_beams;
+        switch (field) {
+            case ORC_F_STATE: memcpy(out + e * A * 7, s->state, sizeof(double) * A * 7); break;
+            case ORC_F_SCANS: memcpy(out + e * A * B, s->scans, sizeof(double) * A * B); break;
+            case ORC_F_SCANS_PRE: memcpy(out + e * A * B, s->scans_pre, sizeof(double) * A * B); break;
+            case ORC_F_COLLISIONS: memcpy(out + e * A, s->collisions, sizeof(double) * A); break;
+            case ORC_F_COLLISION_IDX: memcpy(out + e * A, s->collision_idx, sizeof(double) * A); break;
+            case ORC_F_IN_COLLISION: for (size_t i = 0; i < A; i++) out[e * A + i] = (double)s->in_collision[i]; break;
+            case ORC_F_LAP_TIMES: memcpy(out + e * A, s->lap_times, sizeof(double) * A); break;
+            case ORC_F_LAP_COUNTS: memcpy(out + e * A, s->lap_counts, sizeof(double) * A); break;
+            case ORC_F_TOGGLE_LIST: memcpy(out + e * A, s->toggle_list, sizeof(double) * A); break;
+            case ORC_F_DONE: out[e] = (double)s->done; break;
+            case ORC_F_CURRENT_TIME: out[e] = s->current_time; break;
+            case ORC_F_NLOOK: out[e] = (double)s->nlook; break;
+        }
+    }
 }
 
 /* ------------------------------------------------------------------ batched CPU-baseline driver

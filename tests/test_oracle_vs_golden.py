@@ -129,6 +129,75 @@ def test_trajectories(example_map, name):
         assert n_col > 0
 
 
+@pytest.mark.parametrize('name', ['traj_a1_random', 'traj_a2_random', 'traj_a2_close', 'traj_a3_euler', 'traj_a4_train'])
+def test_step_batch_equals_per_sim_step(example_map, name):
+    """orc_step_batch (the threaded batch driver of the large-batch GPU tests) over the golden trajectories: every field of
+    every env equals the one-sim-at-a-time step, bit for bit, with and without the env-level logic; the optional noise is
+    added to the scan before the opponent ray-cast."""
+    k = g(name + '.npz')
+    E, T, A = k['actions'].shape[:3]
+    kw = dict(num_agents=A, integrator=int(k['integrator']), lidar_dist=float(k['lidar_dist']))
+    one = [oracle.OracleSim(example_map, **kw) for _ in range(E)]
+    bat = [oracle.OracleSim(example_map, **kw) for _ in range(E)]
+    for e in range(E):
+        one[e].env_reset(k['poses0'][e])
+        bat[e].env_reset(k['poses0'][e])
+    for t in range(T):
+        env_level = t % 2 == 1
+        done = []
+        for e in range(E):
+            one[e].step(k['actions'][e, t])
+            done.append(one[e].env_post_step() if env_level else None)
+        oracle.step_batch(bat, k['actions'][:, t], env_level=env_level, num_threads=3)
+        for f in ('state', 'scans', 'collisions', 'collision_idx', 'in_collision', 'lap_times', 'lap_counts', 'toggle_list'):
+            got = oracle.gather(bat, f)
+            want = np.stack([getattr(o, f) for o in one]).astype(np.float64)
+            assert np.array_equal(got, want), (f, t)
+        assert np.array_equal(oracle.gather(bat, 'current_time'), [o.current_time for o in one])
+        assert np.array_equal(oracle.gather(bat, 'nlook'), [o.nlook for o in one])
+        if env_level:
+            assert np.array_equal(oracle.gather(bat, 'done'), np.array(done, dtype=np.float64)), t
+    assert np.array_equal(oracle.gather(bat, 'scans'), oracle.gather(one, 'scans'))
+    # noise: the scan check_ttc and the opponent ray-cast see is the clean one plus the noise (first tick from rest: no
+    # iTTC flag can flip)
+    B = 1080
+    clean = [oracle.OracleSim(example_map, **kw) for _ in range(E)]
+    noisy = [oracle.OracleSim(example_map, **kw) for _ in range(E)]
+    for e in range(E):
+        clean[e].reset(k['poses0'][e])
+        noisy[e].reset(k['poses0'][e])
+    nz = np.random.default_rng(1).normal(0.0, 0.01, (E, A, B))
+    oracle.step_batch(clean, k['actions'][:, 0])
+    oracle.step_batch(noisy, k['actions'][:, 0], noise=nz)
+    assert np.array_equal(oracle.gather(noisy, 'scans_pre'), oracle.gather(clean, 'scans_pre') + nz)
+    assert np.array_equal(oracle.gather(noisy, 'state'), oracle.gather(clean, 'state'))
+    if A == 1:
+        assert np.array_equal(oracle.gather(noisy, 'scans'), oracle.gather(noisy, 'scans_pre'))
+    occl = oracle.gather(noisy, 'scans') < oracle.gather(noisy, 'scans_pre')
+    assert np.array_equal(oracle.gather(noisy, 'scans')[~occl], oracle.gather(noisy, 'scans_pre')[~occl])
+
+
+def test_env_restart_is_the_device_autoreset():
+    """orc_env_restart: Simulator.reset + counters and start frame of F110Env.reset, no zero-action step; done and the
+    collision observation of the ending tick stay."""
+    m = oracle.OracleMap.from_yaml(os.path.join(MAPS, 'example_map.yaml'), '.png')
+    from f1tenth_gym_b200 import maps
+    wp = maps.load_waypoints()
+    s = oracle.OracleSim(m, num_agents=2)
+    s.env_reset(wp[[10, 5]])
+    for _ in range(5):
+        s.step(np.array([[0.3, 6.0], [-0.2, 5.0]]))
+        s.env_post_step()
+    s.collisions[0] = 1.0
+    n0 = s.nlook
+    s.env_restart(wp[[40, 17]])
+    assert np.array_equal(s.state[:, [0, 1, 4]], wp[[40, 17]]) and not s.state[:, [2, 3, 5, 6]].any()
+    assert s.current_time == 0.0 and not s.toggle_list.any() and s.collisions[0] == 1.0
+    assert not s.steer_cnt.any() and s.nlook == n0                  # nothing was stepped
+    s.step(np.zeros((2, 2)))
+    assert not s.env_post_step()                                    # lap logic measured from the new start frame
+
+
 def test_scans_rotated_origin():
     """A map yaml whose origin has a yaw (0.35 rad): the rotation terms of xy_2_rc (laser_models.py:75-78), which none
     of the bundled maps exercises.  Golden: the reference ScanSimulator2D on example_map.png with that origin."""
