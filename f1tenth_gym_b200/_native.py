@@ -12,7 +12,8 @@ LIB_PATH = os.path.join(_HERE, 'libf110_b200.so')
 
 F110_NPARAM = 18
 F110_NSTATE = 7
-ABI_VERSION = 2
+ABI_VERSION = 3
+MAX_START_TABLES = 64
 
 _dp = C.c_void_p   # device / host pointers are passed as raw addresses
 
@@ -27,7 +28,8 @@ class F110Map(C.Structure):
                 ('dt', _dp), ('dt_cells', _dp), ('dt_codes', _dp), ('dt_lut', _dp),
                 ('sines', _dp), ('cosines', _dp), ('sincos', _dp),
                 ('dt_cells_pad', _dp), ('dt_codes_pad', _dp), ('codes_pitch', C.c_uint32), ('sincos2', _dp),
-                ('dt_min_positive', C.c_double), ('num_layers', C.c_int32)]
+                ('dt_min_positive', C.c_double), ('num_layers', C.c_int32),
+                ('layer_geom', _dp), ('layer_orig_max', C.c_double)]
 
 
 class F110Beams(C.Structure):
@@ -50,7 +52,8 @@ class F110Sim(C.Structure):
                 ('start_rot', _dp), ('done', _dp), ('checkpoint_done', _dp), ('env_arrivals', _dp), ('env_layer', _dp),
                 ('lookup_counter', _dp), ('tick_counter', _dp),
                 ('march_cost', _dp), ('march_order', _dp), ('march_count', _dp), ('march_ipa', C.c_int32),
-                ('march_rec', _dp), ('noise_std', C.c_double), ('noise_seed', C.c_uint64)]
+                ('march_rec', _dp), ('noise_std', C.c_double), ('noise_seed', C.c_uint64),
+                ('start_offsets', _dp), ('num_start_tables', C.c_int32)]
 
 
 class F110HostObs(C.Structure):

@@ -5,7 +5,9 @@
 //                                       the march (+ extra blocks that sort last tick's work items into the march queue)
 //   k_march_lean   persistent, warp per 32-beam item (march_lean.cuh): LUT heading, sphere tracing on the DT grid, fused iTTC
 //                                       predicate, optional seeded noise, fp32 range out -- the roofline kernel.  Maps with a
-//                                       rotated origin and stand-alone scans run the literal k_raymarch (thread per beam)
+//                                       rotated origin and stand-alone scans run the literal k_raymarch (thread per beam);
+//                                       canvas stacks of maps with different sizes / origins run k_march_lean_het
+//                                       (march_het.cuh)
 //   k_tail         warp per agent       GJK vs. the other agents of the env, wall-hit state zeroing, opponent ray-cast inside the
 //                                       blocked-view window, collisions obs, then lap logic and auto-reset per env
 //                                       (k_finalize = the same without the env-level part, for f110_step)
@@ -22,6 +24,7 @@
 #include "lidar.cuh"
 #include "march.cuh"
 #include "march_lean.cuh"
+#include "march_het.cuh"
 #include "march_tile.cuh"
 #include "planner.cuh"
 #include "edt.cuh"
@@ -196,6 +199,7 @@ struct FirstLookup {
     double side_max, ttc_margin;
     unsigned long long rec_layer_stride;     // elements between map layers of the table the lean kernel reads
     int agent_queue;                         // 1: the extra blocks build the agent-level queue of the tile march kernel
+    const double *__restrict__ layer_geom;   // canvas stack (f110_map.layer_geom): [L][6] per-layer origin and extent, or NULL
 };
 
 __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__restrict__ actions, double fov,
@@ -239,7 +243,25 @@ __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__re
     // beam of this agent (laser_models.py:129), done once here; otherwise the yaw
     double slot2 = st[4];
     const size_t lo = fl.env_layer ? (size_t)fl.env_layer[a / s.num_agents] * (size_t)fl.layer_stride : (size_t)0;
-    if (fl.cells && !fl.metres) {
+    if (fl.layer_geom) {
+        // canvas stack: the env's own origin and extent; the canvas cells beyond the layer hold its dt[-1,-1], so a column
+        // (row) index up to the canvas width (height) reads what the reference reads off that map
+        const double *__restrict__ g = fl.layer_geom + 6 * (size_t)fl.env_layer[a / s.num_agents];
+        if (!fl.metres) {
+            CellConsts k;
+            k.ox = g[0] * fl.inv_res; k.oy = g[1] * fl.inv_res; k.eps = 0; k.tmax = 0;
+            k.width = fl.width; k.height = fl.height; k.last = fl.last;
+            slot2 = __ldg(fl.cells + lo + cell_index(sx * fl.inv_res, sy * fl.inv_res, k));
+        } else {
+            const double tx = sx - g[0], ty = sy - g[1];
+            unsigned idx = fl.last;
+            if (!(tx < 0 || tx >= g[2] || ty < 0 || ty >= g[3])) {
+                const unsigned c = (unsigned)(int)(tx / fl.res), r = (unsigned)(int)(ty / fl.res);
+                if (c < fl.width && r < fl.height) idx = r * fl.width + c;
+            }
+            slot2 = __ldg(fl.cells + lo + idx);
+        }
+    } else if (fl.cells && !fl.metres) {
         CellConsts k;
         k.ox = fl.ox; k.oy = fl.oy; k.eps = 0; k.tmax = 0; k.width = fl.width; k.height = fl.height; k.last = fl.last;
         slot2 = __ldg(fl.cells + lo + cell_index(sx * fl.inv_res, sy * fl.inv_res, k));
@@ -588,6 +610,8 @@ struct AutoResetArgs {
     const double *start_poses;   // [num_start][3] or NULL = off
     int num_start, pose_gap;
     uint64_t seed, tick_host;
+    int num_tables;              // 0: one shared start table; L: per-layer tables (f110_sim.start_offsets), env_layer set
+    int32_t start_off[F110_MAX_START_TABLES + 1];   // host copy of f110_sim.start_offsets, by value (CUDA graphs keep it)
 };
 
 // one thread per env: reset the env if its ego collided (benchmark / RL convenience, SURVEY.md 8d)
@@ -595,7 +619,13 @@ __device__ __forceinline__ void autoreset_one(const f110_sim &s, int env, const 
     const int A = s.num_agents, NA = s.num_envs * s.num_agents;
     if (s.collisions[(size_t)env * A + s.ego_idx] == 0.0) return;
     const double *__restrict__ start_poses = ar.start_poses;
-    const int num_start = ar.num_start, pose_gap = ar.pose_gap;
+    int num_start = ar.num_start;
+    const int pose_gap = ar.pose_gap;
+    if (ar.num_tables) {         // the start table of the env's own map: rows [start_off[l], start_off[l + 1])
+        const int l = s.env_layer[env];
+        start_poses += 3 * (size_t)ar.start_off[l];
+        num_start = ar.start_off[l + 1] - ar.start_off[l];
+    }
     const uint64_t seed = ar.seed;
     const uint64_t tick = s.tick_counter ? (uint64_t)*s.tick_counter : ar.tick_host;
     uint64_t h = mix64(seed + 0x9E3779B97F4A7C15ull * (tick + 1) + 0xD1B54A32D192ED03ull * (uint64_t)(env + 1));
@@ -1165,6 +1195,27 @@ static void launch_lean(const LeanK &q, const MarchQueue &mq, unsigned sms, bool
     else launch_lean_t<0, true, false, 4>(q, mq, sms * 4u, noise, count, st);
 }
 
+// canvas stacks (march_het.cuh): the block shape rule of the layered lean kernel (static queue, 2 x 1024 threads per SM for
+// long queues, else 4 x 512)
+template <bool CELLS, int PT, int MINB>
+static void launch_het_t(const LeanK &q, const LayerGeomK &g, const MarchQueue &mq, unsigned blocks, int layers, bool noise,
+                         bool count, cudaStream_t st) {
+    const bool pdl = g_pdl_this_step;
+    snprintf(g_launch_march, sizeof(g_launch_march), "march=lean-het HET=1 layers=%d CELLS=%d DYN=0 IPT=1 PT=%d MINB=%d NOISE=%d COUNT=%d grid=%u",
+             layers, CELLS ? 1 : 0, PT, MINB, noise ? 1 : 0, count ? 1 : 0, blocks);
+    if (count) launch_k(k_march_lean_het<false, true, CELLS, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, mq);
+    else if (noise) launch_k(k_march_lean_het<true, false, CELLS, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, mq);
+    else launch_k(k_march_lean_het<false, false, CELLS, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, mq);
+}
+static void launch_het(const LeanK &q, const LayerGeomK &g, const MarchQueue &mq, unsigned sms, bool cells, int layers, bool noise,
+                       bool count, cudaStream_t st) {
+    const bool big = (unsigned long long)mq.items >= 700ull * 2ull * (unsigned long long)sms;
+    if (big && cells) launch_het_t<true, 1024, 2>(q, g, mq, sms * 2u, layers, noise, count, st);
+    else if (big) launch_het_t<false, 1024, 2>(q, g, mq, sms * 2u, layers, noise, count, st);
+    else if (cells) launch_het_t<true, 512, 4>(q, g, mq, sms * 4u, layers, noise, count, st);
+    else launch_het_t<false, 512, 4>(q, g, mq, sms * 4u, layers, noise, count, st);
+}
+
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -1329,7 +1380,11 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     // count: that is exact only while no ray from there can come back onto the map, i.e. the map, a ray's reach
     // (max_range plus one step of at most the map's diagonal) and the origin all stay well inside that bound.  Any other
     // map takes k_raymarch, which has the full row / column checks.
-    const double reach = fmax(fabs(map->orig_x), fabs(map->orig_y)) + 2.0 * (mv.x_max + mv.y_max) + map->max_range;
+    // (a canvas stack: the largest origin of any layer and the canvas extent, which bounds every layer's)
+    const bool het = map->num_layers > 1 && map->layer_geom;
+    const double orig_max = het ? fmax(map->layer_orig_max, fmax(fabs(map->orig_x), fabs(map->orig_y)))
+                                : fmax(fabs(map->orig_x), fabs(map->orig_y));
+    const double reach = orig_max + 2.0 * (mv.x_max + mv.y_max) + map->max_range;
     const bool cell_march = map->orig_c == 1.0 && map->orig_s == 0.0 && map->sincos && beams->cos_side &&
                             (unsigned long long)map->width * (unsigned long long)map->height < (1ull << 32) &&
                             reach < 0.5 * fmin(1e8, 1e9 * map->resolution) && variant != 13;
@@ -1365,6 +1420,9 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     fl.side_max = beams->side_max > 0.0 ? beams->side_max : INFINITY;
     fl.ttc_margin = sim->ttc_thresh * 1.000001;
     fl.rec_layer_stride = cell_units ? (unsigned long long)(map->width + 1) * (unsigned long long)(map->height + 1) : fl.layer_stride;
+    // a canvas stack runs only on the heterogeneous lean kernel (march_het.cuh), one layer per env
+    if (het && (!lean || tile || !layered)) return F110_ERR_INVALID;
+    fl.layer_geom = het ? map->layer_geom : nullptr;
     k_dynamics<<<dyn_blocks + order_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, dyn_blocks, fl);
     LAUNCH_CHECK("k_dynamics");
     if (ev) CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -1468,6 +1526,10 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
                 t.c_max = (int)map->codes_pitch - tile_sz; t.r_max = map->height + 1 - tile_sz;
                 t.tile_counter = g_tile_counter;
                 if ((rc = launch_tile(t, map, tile_sz, (unsigned)num_sms(), noise, count, st))) return rc;
+            } else if (het) {
+                LayerGeomK g;
+                g.layer_geom = map->layer_geom; g.env_layer = sim->env_layer; g.num_agents = (unsigned)sim->num_agents;
+                launch_het(q, g, mq, (unsigned)num_sms(), cell_units, map->num_layers, noise, count, st);
             } else
             launch_lean(q, mq, (unsigned)num_sms(), cell_units, lcoded, occ3, layered, noise, count,
                         /* dynamic queue tail: */ (variant == 0 || variant == 40 || variant == 41 || variant == 42 || variant == 43 || variant == 45 || variant == 57 || variant == 58 || (variant >= 81 && variant <= 86)) && !layered &&
@@ -1515,6 +1577,7 @@ marched:
         int epb = g_tail2_forced ? max(1, g_tail2_agents / sim->num_agents) : max(1, min(g_tail2_agents / sim->num_agents, sim->num_envs / (4 * num_sms())));
         AutoResetArgs no_ar;
         no_ar.start_poses = nullptr; no_ar.num_start = 0; no_ar.pose_gap = 0; no_ar.seed = 0; no_ar.tick_host = 0;
+        no_ar.num_tables = 0;
         const bool fused = tail && tail->fused;
         // big blocks (>= 48 agents) run 256 threads, small ones 128 (measured: 256:64 best at cfg3, 128:12 at cfg2x2)
         int t2 = (g_tail2_threads != F110_TAIL2_THREADS) ? g_tail2_threads : (epb * sim->num_agents >= 48 ? 256 : 128);
@@ -1571,8 +1634,8 @@ marched:
             if (tail->ar.start_poses) { k_autoreset<<<(sim->num_envs + 127) / 128, 128, 0, st>>>(*sim, tail->ar); LAUNCH_CHECK("k_autoreset"); }
         }
     }
-    snprintf(g_launch_rec, sizeof(g_launch_rec), "%s static_runs=%u per_warp=%u %s", g_launch_march, rec_static_runs, rec_per_warp,
-             rec_tail);
+    snprintf(g_launch_rec, sizeof(g_launch_rec), "%s%s static_runs=%u per_warp=%u %s", g_launch_march, het ? "" : " HET=0",
+             rec_static_runs, rec_per_warp, rec_tail);
     if (ev) CUDA_TRY(cudaEventRecord(ev[3], st));
     return F110_OK;
 }
@@ -1635,6 +1698,21 @@ int f110_env_post_step(const f110_sim *sim, void *stream) {
     return F110_OK;
 }
 
+// per-layer start tables (f110_sim.start_offsets, host memory) -> ar.num_tables / ar.start_off; no tables without env_layer
+static int start_tables(const f110_sim *sim, int32_t num_start, AutoResetArgs &ar) {
+    ar.num_tables = 0;
+    if (!sim->start_offsets || !sim->env_layer) return F110_OK;
+    const int L = sim->num_start_tables;
+    if (L < 1 || L > F110_MAX_START_TABLES || sim->start_offsets[0] != 0 || sim->start_offsets[L] != num_start)
+        return F110_ERR_INVALID;
+    for (int l = 0; l <= L; l++) {
+        if (l < L && sim->start_offsets[l + 1] <= sim->start_offsets[l]) return F110_ERR_INVALID;
+        ar.start_off[l] = sim->start_offsets[l];
+    }
+    ar.num_tables = L;
+    return F110_OK;
+}
+
 int f110_autoreset(const f110_sim *sim, const double *start_poses, int32_t num_start, int32_t pose_gap,
                    uint64_t seed, uint64_t tick, void *stream) {
     int rc;
@@ -1644,6 +1722,7 @@ int f110_autoreset(const f110_sim *sim, const double *start_poses, int32_t num_s
     if (sim->num_agents > 32) return F110_ERR_INVALID;      // the device-side auto-reset stages at most 32 start poses per env
     AutoResetArgs ar;
     ar.start_poses = start_poses; ar.num_start = num_start; ar.pose_gap = pose_gap; ar.seed = seed; ar.tick_host = tick;
+    if ((rc = start_tables(sim, num_start, ar))) return rc;
     k_autoreset<<<(sim->num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*sim, ar);
     LAUNCH_CHECK("k_autoreset");
     return F110_OK;
@@ -1660,6 +1739,9 @@ int f110_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams,
     TailOpts t;
     t.fused = true; t.env_level = env_level;
     t.ar.start_poses = start_poses; t.ar.num_start = num_start; t.ar.pose_gap = pose_gap; t.ar.seed = seed; t.ar.tick_host = 0;
+    t.ar.num_tables = 0;
+    if (start_poses && (rc = start_tables(sim, num_start, t.ar))) return rc;
+    if (t.ar.num_tables && (!map || t.ar.num_tables != map->num_layers)) return F110_ERR_INVALID;
     return step_impl(sim, map, beams, actions, (cudaStream_t)stream, nullptr, &t);
 }
 
@@ -1745,6 +1827,7 @@ int f110_scan(const f110_map *map, const f110_beams *beams, const double *poses,
     int rc;
     if ((rc = check_map(map)) || (rc = check_beams(beams))) return rc;
     if (!poses || M <= 0 || (!out_f32 && !out_f64)) return F110_ERR_INVALID;
+    if (map->num_layers > 1 && map->layer_geom) return F110_ERR_INVALID;     // canvas stacks: the tick only
     MarchArgs g;
     memset(&g, 0, sizeof(g));
     g.scan_pose = poses;

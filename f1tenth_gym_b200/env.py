@@ -10,6 +10,8 @@ params=<18-key dict>, num_agents=2, timestep=0.01, ego_idx=0, integrator=RK4, li
 Extensions: num_envs (None = single env, reference-shaped numpy/list outputs; int = batched torch
 tensors (N,A,...) that are views of device buffers valid until the next step), num_beams, fov, device,
 scan_noise_std (reference default 0.01; 0 disables the noise for bit-reproducible parity runs).
+Batched mode also takes a list of maps, map=['berlin', 'vegas', ...] with map_ext one extension or a list, stacked into
+one simulator (DeviceMap.stack: one resolution, unrotated origins); env e drives on map env_map_ids[e] (default e % L).
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
@@ -27,7 +29,10 @@ class F110Env(object):
         self.seed = kwargs.get('seed', 12345)
         if 'map' in kwargs:
             self.map_name = kwargs['map']
-            self.map_path = hostmaps.resolve_map_path(self.map_name)
+            if isinstance(self.map_name, (list, tuple)):
+                self.map_path = [hostmaps.resolve_map_path(m) for m in self.map_name]
+            else:
+                self.map_path = hostmaps.resolve_map_path(self.map_name)
         else:
             self.map_name = 'vegas'
             self.map_path = hostmaps.resolve_map_path('vegas')
@@ -41,13 +46,16 @@ class F110Env(object):
         num_envs = kwargs.get('num_envs', None)
         self.batched = num_envs is not None
         self.num_envs = int(num_envs) if self.batched else 1
+        if isinstance(self.map_path, (list, tuple)) and not self.batched:
+            raise ValueError('a list of maps needs the batched mode (num_envs)')
         self.start_thresh = 0.5
         self.sim = Simulator(self.params, self.num_agents, self.seed, time_step=self.timestep,
                              ego_idx=self.ego_idx, integrator=self.integrator, lidar_dist=self.lidar_dist,
                              num_envs=self.num_envs, num_beams=kwargs.get('num_beams', 1080),
                              fov=kwargs.get('fov', 4.7), device=kwargs.get('device', None),
                              noise_std=kwargs.get('scan_noise_std', 0.01))
-        self.sim.set_map(self.map_path, self.map_ext)
+        self.env_map_ids = kwargs.get('env_map_ids', None)
+        self._set_map(self.map_path, self.map_ext)
         self.render_obs = None
         # single-env mode: the whole observation comes back in ONE batch of async copies + one stream sync
         # (C ABI f110_step_host) instead of a blocking .cpu() per field
@@ -136,9 +144,34 @@ class F110Env(object):
         """Batch extension: re-initialise only the masked envs (counters + Simulator.reset); no tick is run."""
         self.sim.env_reset(poses, env_mask)
 
-    def update_map(self, map_path, map_ext):
-        """f110_env.py:351-362"""
-        self.sim.set_map(map_path, map_ext)
+    def update_map(self, map_path, map_ext, env_map_ids=None):
+        """f110_env.py:351-362.  Batch extension: lists of map paths (and extensions) as in the constructor."""
+        if env_map_ids is not None:
+            self.env_map_ids = env_map_ids
+        self._set_map(map_path, map_ext)
+
+    def _set_map(self, map_path, map_ext):
+        """One map, or (batched mode) a list of maps stacked into one DeviceMap; env e drives on map env_map_ids[e]
+        (default e % L) and auto-resets from that map's start table when Simulator.tick gets one table per map."""
+        if not isinstance(map_path, (list, tuple)):
+            self.sim.set_map(map_path, map_ext)
+            return
+        if not self.batched:
+            raise ValueError('a list of maps needs the batched mode (num_envs)')
+        exts = list(map_ext) if isinstance(map_ext, (list, tuple)) else [map_ext] * len(map_path)
+        if len(exts) != len(map_path) or len(map_path) < 1:
+            raise ValueError('map_ext must be one extension or one per map')
+        from .simulator import DeviceMap
+        layers = [DeviceMap.from_yaml(p, e, self.sim.device) for p, e in zip(map_path, exts)]
+        ids = self.env_map_ids
+        if ids is None:
+            ids = np.arange(self.num_envs) % len(layers)
+        if len(layers) == 1:
+            if np.any(np.asarray(ids) != 0):
+                raise ValueError('env_map_ids must index the list of maps')
+            self.sim.set_device_map(layers[0])
+        else:
+            self.sim.set_device_map(DeviceMap.stack(layers), env_map_ids=ids)
 
     def update_params(self, params, index=-1):
         """f110_env.py:364-375"""

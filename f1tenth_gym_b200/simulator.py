@@ -87,14 +87,15 @@ class DeviceMap(object):
 
     @classmethod
     def stack(cls, maps):
-        """Multi-map batch (SURVEY 8f row 3): several DeviceMaps that share size, resolution and origin are
-        stacked into one [L][H][W] table; Simulator.set_device_map(stacked, env_map_ids) picks one per env."""
+        """Multi-map batch (SURVEY 8f row 3): Simulator.set_device_map(stacked, env_map_ids) picks one layer per env.
+        Maps that share size, resolution and origin are stacked into one [L][H][W] table.  Other unrotated maps of one
+        resolution are stacked on a canvas (see _stack_canvas); mixed resolutions and rotated origins raise ValueError."""
         m0 = maps[0]
-        for m in maps[1:]:
-            h, h0 = m.host, m0.host
-            if (h.height, h.width, h.resolution, h.orig_x, h.orig_y, h.orig_c, h.orig_s) != \
-               (h0.height, h0.width, h0.resolution, h0.orig_x, h0.orig_y, h0.orig_c, h0.orig_s):
-                raise ValueError('stacked maps must share size, resolution and origin')
+        h0 = m0.host
+        key0 = (h0.height, h0.width, h0.resolution, h0.orig_x, h0.orig_y, h0.orig_c, h0.orig_s)
+        if any((m.host.height, m.host.width, m.host.resolution, m.host.orig_x, m.host.orig_y, m.host.orig_c,
+                m.host.orig_s) != key0 for m in maps[1:]):
+            return cls._stack_canvas(maps)
         out = cls.__new__(cls)
         out.__dict__.update(m0.__dict__)
         out.layers = list(maps)
@@ -111,6 +112,56 @@ class DeviceMap(object):
         c.dt_codes_pad = None
         c.num_layers = len(maps)
         c.dt_min_positive = min(m.c.dt_min_positive for m in maps)
+        out.c = c
+        return out
+
+    @classmethod
+    def _stack_canvas(cls, maps):
+        """Maps of different size and origin on one [L][Hc][Wc] canvas (Wc = max W_l, Hc = max H_l): layer l's table sits in
+        the low corner of its slice and every other cell of the slice holds that layer's dt[-1,-1], which is what the
+        reference reads off that map, so the march kernels clamp to the canvas and need no per-layer width or height.  The
+        cell-unit padded table gets the same treatment with its extra row and column.  f110_map.layer_geom carries each
+        layer's (orig_x, orig_y, x_max = W_l * res, y_max = H_l * res, W_l, H_l)."""
+        hs = [m.host for m in maps]
+        h0 = hs[0]
+        if any(h.resolution != h0.resolution for h in hs):
+            raise ValueError('stacked maps must share one resolution')
+        if any(h.orig_c != 1.0 or h.orig_s != 0.0 for h in hs):
+            raise ValueError('stacked maps of different size or origin need unrotated origins')
+        if any((m.dt_cells is None) != (maps[0].dt_cells is None) for m in maps):
+            raise ValueError('stacked maps must all have, or all lack, the cell-unit table')
+        L = len(maps)
+        Hc, Wc = max(h.height for h in hs), max(h.width for h in hs)
+
+        def canvas(tables, extra):
+            out = torch.empty((L, Hc + extra, Wc + extra), dtype=tables[0].dtype, device=tables[0].device)
+            for l, t in enumerate(tables):
+                out[l] = t[-1, -1]
+                out[l, :t.shape[0], :t.shape[1]] = t
+            return out.contiguous()
+        out = cls.__new__(cls)
+        out.__dict__.update(maps[0].__dict__)
+        out.layers = list(maps)
+        out.dt = canvas([m.dt for m in maps], 0)
+        out.dt_cells = canvas([m.dt_cells for m in maps], 0) if maps[0].dt_cells is not None else None
+        out.dt_cells_pad = canvas([m.dt_cells for m in maps], 1) if maps[0].dt_cells is not None else None
+        out.dt_codes = out.dt_lut = out.dt_codes_pad = None
+        out.layer_geom_host = np.array([[h.orig_x, h.orig_y, h.width * h.resolution, h.height * h.resolution, h.width,
+                                         h.height] for h in hs], dtype=np.float64)
+        out.layer_geom = torch.from_numpy(out.layer_geom_host).to(maps[0].device)
+        c = nat.F110Map.from_buffer_copy(maps[0].c)
+        c.height, c.width = Hc, Wc
+        c.dt = nat.ptr(out.dt)
+        c.dt_cells = nat.ptr(out.dt_cells)
+        c.dt_cells_pad = nat.ptr(out.dt_cells_pad)
+        c.dt_codes = None
+        c.dt_lut = None
+        c.dt_codes_pad = None
+        c.codes_pitch = 0
+        c.num_layers = L
+        c.dt_min_positive = min(m.c.dt_min_positive for m in maps)
+        c.layer_geom = nat.ptr(out.layer_geom)
+        c.layer_orig_max = float(np.abs(out.layer_geom_host[:, :2]).max())
         out.c = c
         return out
 
@@ -223,6 +274,7 @@ class Simulator(object):
         self.march_rec = torch.zeros((NA, 8), **f64) if self.march_ipa else None
         self.beams = DeviceBeams(num_beams, fov, params, dev)
         self.map = None
+        self.env_layer = None
         self._map_struct = empty_map_struct()
         self._actions_dev = torch.zeros((NA, 2), **f64)
         self.c = nat.F110Sim(
@@ -362,18 +414,41 @@ class Simulator(object):
         """Tail of F110Env.step: time + lap logic + done (f110_env.py:294-302, 204-246)."""
         nat.check(nat.lib().f110_env_post_step(C.byref(self.c), _stream_ptr(self.device)))
 
+    def _start_table(self, poses):
+        """Auto-reset start poses -> (device (K,3) table, K).  `poses` is one (K,3) device tensor shared by every env, or, for
+        a stacked DeviceMap, a list of one (K_l,3) table per layer: they are concatenated on the device and
+        f110_sim.start_offsets is set so that an env restarts from its own map's table."""
+        self.c.start_offsets = None
+        self.c.num_start_tables = 0
+        if poses is None:
+            return None, 0
+        if not isinstance(poses, (list, tuple)):
+            return poses, poses.shape[0]
+        layers = getattr(self._map_struct, 'num_layers', 1)
+        if layers <= 1 or self.env_layer is None or len(poses) != layers:
+            raise ValueError('autoreset_poses as a list needs one start table per layer of the stacked map (%d)'
+                             % max(layers, 1))
+        tabs = [torch.as_tensor(p, dtype=torch.float64).to(self.device).reshape(-1, 3) for p in poses]
+        offs = np.concatenate([[0], np.cumsum([t.shape[0] for t in tabs])]).astype(np.int32)
+        self._start_offsets = (C.c_int32 * offs.size)(*offs.tolist())
+        self.c.start_offsets = C.addressof(self._start_offsets)
+        self.c.num_start_tables = layers
+        return torch.cat(tabs).contiguous(), int(offs[-1])
+
     def autoreset(self, start_poses, pose_gap=23, seed=12345):
-        """Reset every env whose ego collided to a hashed draw from start_poses (device (K,3) fp64)."""
-        nat.check(nat.lib().f110_autoreset(C.byref(self.c), nat.ptr(start_poses), start_poses.shape[0],
-                                           pose_gap, int(seed), 0, _stream_ptr(self.device)))
+        """Reset every env whose ego collided to a hashed draw from start_poses (device (K,3) fp64, or a list of one
+        (K_l,3) table per layer of a stacked map)."""
+        table, n = self._start_table(start_poses)
+        nat.check(nat.lib().f110_autoreset(C.byref(self.c), nat.ptr(table), n, pose_gap, int(seed), 0,
+                                           _stream_ptr(self.device)))
 
     def tick(self, control_inputs, env_level=True, autoreset_poses=None, pose_gap=23, seed=12345):
         """One whole tick in three launches (C ABI f110_tick): step + lap logic + optional auto-reset, same
         results as step(); env_post_step(); autoreset()."""
         a = self._actions_tensor(control_inputs)
-        n = 0 if autoreset_poses is None else autoreset_poses.shape[0]
+        table, n = self._start_table(autoreset_poses)
         nat.check(nat.lib().f110_tick(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c), nat.ptr(a),
-                                      1 if env_level else 0, nat.ptr(autoreset_poses), n, pose_gap, int(seed),
+                                      1 if env_level else 0, nat.ptr(table), n, pose_gap, int(seed),
                                       _stream_ptr(self.device)))
         return self.observations()
 
@@ -401,11 +476,11 @@ class Simulator(object):
                  'start_ys', 'start_thetas', 'start_rot', 'done', 'checkpoint_done', 'tick_counter', 'march_cost',
                  'march_order', 'march_count', 'march_rec')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
+        table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
 
         def tick():
-            n = 0 if autoreset_poses is None else autoreset_poses.shape[0]
             nat.check(L.f110_tick(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c), nat.ptr(actions),
-                                  1 if env_level else 0, nat.ptr(autoreset_poses), n, pose_gap, int(autoreset_seed),
+                                  1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(autoreset_seed),
                                   _stream_ptr(self.device)))
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
@@ -420,7 +495,7 @@ class Simulator(object):
         with torch.cuda.graph(g):
             tick()
         self._graph = g
-        self._graph_keep = (actions, autoreset_poses)
+        self._graph_keep = (actions, table)
         return g
 
     def replay(self):

@@ -25,10 +25,11 @@
 extern "C" {
 #endif
 
-#define F110_ABI_VERSION 2
+#define F110_ABI_VERSION 3
 #define F110_NPARAM 18     /* mu C_Sf C_Sr lf lr h m I s_min s_max sv_min sv_max v_switch a_max v_min v_max width length
                               (key order of the default dict, f110_env.py:130) */
 #define F110_NSTATE 7      /* x y steer v yaw yaw_rate slip   (base_classes.py:97) */
+#define F110_MAX_START_TABLES 64   /* per-layer auto-reset start tables (f110_sim.start_offsets) */
 
 typedef enum {
     F110_OK = 0,
@@ -71,6 +72,15 @@ typedef struct {
                                        lean march kernel (csrc/march_lean.cuh) may be used */
     int32_t num_layers;             /* 0/1: one map.  L > 1: dt and dt_cells hold L stacked [H][W] tables that share size,
                                        resolution and origin (multi-map batches); f110_sim.env_layer picks one per env */
+    /* ABI v3 */
+    const double *layer_geom;       /* [num_layers][6] (orig_x, orig_y, x_max = W_l*res, y_max = H_l*res, W_l, H_l) of each layer
+                                       of a canvas stack, or NULL (every layer has the geometry above).  When set, height / width
+                                       are the canvas (max H_l, max W_l); layer l's table sits in the low corner of its canvas
+                                       slice and every other cell of the slice (and of the extra row / column of dt_cells_pad)
+                                       holds that layer's dt[-1,-1].  Unrotated origins and one resolution only; needs the lean
+                                       march kernels (F110_ERR_INVALID otherwise) */
+    double layer_orig_max;          /* with layer_geom: max over the layers of max(|orig_x|, |orig_y|), a host copy for the
+                                       launch-time bound on absurd coordinates (the table itself is device memory) */
 } f110_map;
 
 /* Beam tables RaceCar.__init__ builds once (base_classes.py:122-158) + ScanSimulator2D.__init__ (:360-368). */
@@ -127,6 +137,14 @@ typedef struct {
     /* scan noise (laser_models.py:429,450-452): N(0, noise_std^2) per beam, added before iTTC; 0 = off */
     double noise_std;
     uint64_t noise_seed;
+    /* ABI v3 */
+    const int32_t *start_offsets;   /* [num_start_tables + 1] in HOST memory (read when the auto-reset is enqueued, so a captured
+                                       CUDA graph keeps the values it was captured with), or NULL: with env_layer set, an env on
+                                       layer l auto-resets from rows [start_offsets[l], start_offsets[l+1]) of start_poses (one start
+                                       table per map).  start_offsets[0] == 0, num_start == start_offsets[num_start_tables], every
+                                       range non-empty, at most F110_MAX_START_TABLES tables, and f110_step / f110_tick need
+                                       num_start_tables == the map's num_layers: F110_ERR_INVALID otherwise */
+    int32_t num_start_tables;       /* number of ranges in start_offsets (= num_layers of the map) */
 } f110_sim;
 
 int f110_abi_version(void);
@@ -163,7 +181,9 @@ int f110_env_post_step(const f110_sim *sim, void *stream);
  * What the caller sees after a tick that ended an episode: done[env] = 1 and collisions / scans of the crash
  * (the finished episode's last observation), while state, steer FIFO, lap counters, toggles and current_time are
  * those of the NEW episode (a car at rest on its start pose, time 0); done is recomputed by the next tick.
- * At most 32 agents per env (F110_ERR_INVALID otherwise; stepping itself has no such limit). */
+ * At most 32 agents per env (F110_ERR_INVALID otherwise; stepping itself has no such limit).
+ * Per-map start tables (sim->start_offsets set, sim->env_layer set): the same draw inside the env's layer range,
+ * k = min(floor(u * K_l), K_l - 1), agent i takes start_poses[start_l + (k - pose_gap*i) mod K_l]. */
 int f110_autoreset(const f110_sim *sim, const double *start_poses, int32_t num_start, int32_t pose_gap,
                    uint64_t seed, uint64_t tick, void *stream);
 
