@@ -200,6 +200,7 @@ struct FirstLookup {
     unsigned long long rec_layer_stride;     // elements between map layers of the table the lean kernel reads
     int agent_queue;                         // 1: the extra blocks build the agent-level queue of the tile march kernel
     const double *__restrict__ layer_geom;   // canvas stack (f110_map.layer_geom): [L][6] per-layer origin and extent, or NULL
+    const double *__restrict__ layer_res;    // canvas stack of several resolutions (f110_map.layer_res): [L][2], or NULL
 };
 
 __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__restrict__ actions, double fov,
@@ -254,9 +255,11 @@ __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__re
             slot2 = __ldg(fl.cells + lo + cell_index(sx * fl.inv_res, sy * fl.inv_res, k));
         } else {
             const double tx = sx - g[0], ty = sy - g[1];
+            // the layer's own resolution when the layers differ in it (the reference's IEEE division by that map's res)
+            const double res = fl.layer_res ? fl.layer_res[2 * (size_t)fl.env_layer[a / s.num_agents]] : fl.res;
             unsigned idx = fl.last;
             if (!(tx < 0 || tx >= g[2] || ty < 0 || ty >= g[3])) {
-                const unsigned c = (unsigned)(int)(tx / fl.res), r = (unsigned)(int)(ty / fl.res);
+                const unsigned c = (unsigned)(int)(tx / res), r = (unsigned)(int)(ty / res);
                 if (c < fl.width && r < fl.height) idx = r * fl.width + c;
             }
             slot2 = __ldg(fl.cells + lo + idx);
@@ -1215,6 +1218,23 @@ static void launch_het(const LeanK &q, const LayerGeomK &g, const MarchQueue &mq
     else if (cells) launch_het_t<true, 512, 4>(q, g, mq, sms * 4u, layers, noise, count, st);
     else launch_het_t<false, 512, 4>(q, g, mq, sms * 4u, layers, noise, count, st);
 }
+// canvas stacks of several resolutions (f110_map.layer_res): metres only, the same block shape rule
+template <int PT, int MINB>
+static void launch_het_res_t(const LeanK &q, const LayerGeomK &g, const double *layer_res, const MarchQueue &mq, unsigned blocks,
+                             int layers, bool noise, bool count, cudaStream_t st) {
+    const bool pdl = g_pdl_this_step;
+    snprintf(g_launch_march, sizeof(g_launch_march), "march=lean-het HET=1 layers=%d RES=1 CELLS=0 DYN=0 IPT=1 PT=%d MINB=%d NOISE=%d COUNT=%d grid=%u",
+             layers, PT, MINB, noise ? 1 : 0, count ? 1 : 0, blocks);
+    if (count) launch_k(k_march_lean_het_res<false, true, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, layer_res, mq);
+    else if (noise) launch_k(k_march_lean_het_res<true, false, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, layer_res, mq);
+    else launch_k(k_march_lean_het_res<false, false, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, layer_res, mq);
+}
+static void launch_het_res(const LeanK &q, const LayerGeomK &g, const double *layer_res, const MarchQueue &mq, unsigned sms,
+                           int layers, bool noise, bool count, cudaStream_t st) {
+    if ((unsigned long long)mq.items >= 700ull * 2ull * (unsigned long long)sms)
+        launch_het_res_t<1024, 2>(q, g, layer_res, mq, sms * 2u, layers, noise, count, st);
+    else launch_het_res_t<512, 4>(q, g, layer_res, mq, sms * 4u, layers, noise, count, st);
+}
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
@@ -1382,12 +1402,20 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     // map takes k_raymarch, which has the full row / column checks.
     // (a canvas stack: the largest origin of any layer and the canvas extent, which bounds every layer's)
     const bool het = map->num_layers > 1 && map->layer_geom;
+    // (a canvas stack of several resolutions: the extents at the coarsest layer resolution, the cell bound at the finest;
+    // metres only, on the lean canvas-stack kernel)
+    if (map->layer_res && (!het || map->fast_path || !(map->layer_res_min > 0.0) || !(map->layer_res_max >= map->layer_res_min)))
+        return F110_ERR_INVALID;
+    const bool mixres = het && map->layer_res;
+    const double res_fine = mixres ? map->layer_res_min : map->resolution;
+    const double x_ext = mixres ? map->width * map->layer_res_max : mv.x_max;
+    const double y_ext = mixres ? map->height * map->layer_res_max : mv.y_max;
     const double orig_max = het ? fmax(map->layer_orig_max, fmax(fabs(map->orig_x), fabs(map->orig_y)))
                                 : fmax(fabs(map->orig_x), fabs(map->orig_y));
-    const double reach = orig_max + 2.0 * (mv.x_max + mv.y_max) + map->max_range;
+    const double reach = orig_max + 2.0 * (x_ext + y_ext) + map->max_range;
     const bool cell_march = map->orig_c == 1.0 && map->orig_s == 0.0 && map->sincos && beams->cos_side &&
                             (unsigned long long)map->width * (unsigned long long)map->height < (1ull << 32) &&
-                            reach < 0.5 * fmin(1e8, 1e9 * map->resolution) && variant != 13;
+                            reach < 0.5 * fmin(1e8, 1e9 * res_fine) && variant != 13;
     const bool cell_units = cell_march && map->fast_path && map->dt_cells;
     FirstLookup fl;
     fl.cells = cell_march ? (cell_units ? map->dt_cells : map->dt) : nullptr;
@@ -1398,7 +1426,7 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     if (map->num_layers > 1 && !cell_march) return F110_ERR_INVALID;     // stacked maps need the lean march kernels
     fl.env_layer = layered ? sim->env_layer : nullptr;
     fl.layer_stride = (unsigned long long)map->width * (unsigned long long)map->height;
-    fl.inv_res = 1.0 / map->resolution; fl.ox = map->orig_x * fl.inv_res; fl.oy = map->orig_y * fl.inv_res;
+    fl.inv_res = 1.0 / res_fine; fl.ox = map->orig_x * fl.inv_res; fl.oy = map->orig_y * fl.inv_res;
     fl.width = (unsigned)map->width; fl.height = (unsigned)map->height;
     fl.last = (unsigned)map->width * (unsigned)map->height - 1u;
     // the lean march kernel (march_lean.cuh): 32-beam queue items, `d > eps` == `d != 0` (every positive DT value exceeds
@@ -1423,6 +1451,7 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     // a canvas stack runs only on the heterogeneous lean kernel (march_het.cuh), one layer per env
     if (het && (!lean || tile || !layered)) return F110_ERR_INVALID;
     fl.layer_geom = het ? map->layer_geom : nullptr;
+    fl.layer_res = mixres ? map->layer_res : nullptr;
     k_dynamics<<<dyn_blocks + order_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, dyn_blocks, fl);
     LAUNCH_CHECK("k_dynamics");
     if (ev) CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -1529,7 +1558,8 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
             } else if (het) {
                 LayerGeomK g;
                 g.layer_geom = map->layer_geom; g.env_layer = sim->env_layer; g.num_agents = (unsigned)sim->num_agents;
-                launch_het(q, g, mq, (unsigned)num_sms(), cell_units, map->num_layers, noise, count, st);
+                if (mixres) launch_het_res(q, g, map->layer_res, mq, (unsigned)num_sms(), map->num_layers, noise, count, st);
+                else launch_het(q, g, mq, (unsigned)num_sms(), cell_units, map->num_layers, noise, count, st);
             } else
             launch_lean(q, mq, (unsigned)num_sms(), cell_units, lcoded, occ3, layered, noise, count,
                         /* dynamic queue tail: */ (variant == 0 || variant == 40 || variant == 41 || variant == 42 || variant == 43 || variant == 45 || variant == 57 || variant == 58 || (variant >= 81 && variant <= 86)) && !layered &&
@@ -1827,7 +1857,7 @@ int f110_scan(const f110_map *map, const f110_beams *beams, const double *poses,
     int rc;
     if ((rc = check_map(map)) || (rc = check_beams(beams))) return rc;
     if (!poses || M <= 0 || (!out_f32 && !out_f64)) return F110_ERR_INVALID;
-    if (map->num_layers > 1 && map->layer_geom) return F110_ERR_INVALID;     // canvas stacks: the tick only
+    if ((map->num_layers > 1 && map->layer_geom) || map->layer_res) return F110_ERR_INVALID;     // canvas stacks: the tick only
     MarchArgs g;
     memset(&g, 0, sizeof(g));
     g.scan_pose = poses;

@@ -140,4 +140,109 @@ __global__ void __launch_bounds__(PT, MINB) k_march_lean_het(const LeanK p, cons
     }
 }
 
+// k_march_lean_het_res: a canvas stack whose layers also differ in resolution (f110_map.layer_res), metres only.  The metre
+// loop of k_march_lean_het with the layer's own (res_l, RN(1/res_l)) in the quotient and in march_generic, loaded once per
+// work item next to the origin and extent.  floor(RN(t / res_l)) through the FMA-corrected quotient is the reference's
+// floor(t / res_l) at every resolution (test_boundary_inputs), so each layer keeps the single-map results.  A kernel of its
+// own, not a template argument of k_march_lean_het, so that the existing instances keep their code and their names.
+template <bool NOISE, bool COUNT, int PT, int MINB>
+__global__ void __launch_bounds__(PT, MINB) k_march_lean_het_res(const LeanK p, const LayerGeomK g,
+                                                                 const double *__restrict__ layer_res, const MarchQueue mq) {
+    __shared__ unsigned s_next;
+    if (threadIdx.x == 0) s_next = 0u;
+    pdl_wait();
+    pdl_launch_dependents();
+    __syncthreads();
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned nA = min(mq.count[0], mq.items), nB = min(mq.count[1], mq.items);
+    const unsigned nAB = nA + nB;
+    const unsigned total = min(nAB + min(mq.count[2], mq.items), mq.items);
+    const unsigned cs = mq.chunk_shift;
+    const unsigned qstride = gridDim.x << cs, qbase = blockIdx.x << cs, qmask = (1u << cs) - 1u;
+    const unsigned s_next_addr = (unsigned)__cvta_generic_to_shared(&s_next);
+    unsigned looks = 0u;
+    for (;;) {
+        unsigned k = 0, leader;
+        asm volatile("{\n\t.reg .pred p;\n\telect.sync %1|p, 0xffffffff;\n\t@p atom.shared.add.u32 %0, [%2], 1;\n\t}"
+                     : "+r"(k), "=r"(leader) : "r"(s_next_addr) : "memory");
+        k = __shfl_sync(0xffffffffu, k, leader);
+        const unsigned q = (k >> cs) * qstride + qbase + (k & qmask);
+        if (q >= total) break;
+        const unsigned it = mq.order[(q < nA) ? q : (q < nAB) ? (mq.items + (q - nA)) : (2u * mq.items + (q - nAB))];
+        const unsigned a = it >> 8;
+        const int i = (int)((it & 255u) * 32u + lane);
+        const double2 *__restrict__ rp = p.rec + 4 * (size_t)a;
+        const double2 r0 = __ldg(rp), r1 = __ldg(rp + 1);
+        const unsigned long long ti0fx = (unsigned long long)__double_as_longlong(r1.y);
+        // the agent's map layer: origin, extent and resolution (warp-uniform loads, once per item)
+        const unsigned l = (unsigned)__ldg(g.env_layer + a / g.num_agents);
+        const double *__restrict__ lg = g.layer_geom + 6 * (size_t)l;
+        const double2 lorig = __ldg(reinterpret_cast<const double2 *>(lg));
+        const double2 lres = __ldg(reinterpret_cast<const double2 *>(layer_res) + l);     // (res_l, RN(1 / res_l))
+        unsigned n = 0;
+        if (i < p.B) {
+            double range;
+            const double2 lmax = __ldg(reinterpret_cast<const double2 *>(lg) + 1);
+            if (ti0fx != ~0ull) {
+                const unsigned long long vfx = ti0fx + (unsigned long long)(unsigned)i * p.inc_fx;
+                unsigned ti = (unsigned)(vfx >> F110_FX_SHIFT);
+                const unsigned fr = (unsigned)(vfx >> (F110_FX_SHIFT - 32));
+                if (fr + p.guard32 <= 2u * p.guard32)
+                    ti = (unsigned)replay_theta_index(__ldg(rp + 3).y, i, p.inc, p.theta_dis_f);
+                const double2 sc = __ldg(p.sincos2 + ti);
+                const double *__restrict__ table = p.table + (unsigned long long)__double_as_longlong(__ldg(rp + 3).x);
+                asm volatile("" : "+l"(table));
+                const double MAGIC = 6755399441055744.0;   // 2^52 + 2^51: round-down add == floor in the low word
+                double X = r0.x, Y = r0.y, T = r1.x, D = r1.x;
+                n = 1;
+                if (__double2hiint(D) != 0 && T <= p.tmax) {
+#pragma unroll 1
+                    do {
+                        X = X + D * sc.y;
+                        Y = Y + D * sc.x;
+                        const double tx = X - lorig.x, ty = Y - lorig.y;
+                        double qx = tx * lres.y, qy = ty * lres.y;
+                        qx = __fma_rn(__fma_rn(-qx, lres.x, tx), lres.y, qx);     // RN(tx / res_l), see march.cuh
+                        qy = __fma_rn(__fma_rn(-qy, lres.x, ty), lres.y, qy);
+                        const int c = __double2loint(__dadd_rd(qx, MAGIC));
+                        const int r = __double2loint(__dadd_rd(qy, MAGIC));
+                        unsigned idx = (unsigned)r * p.width + (unsigned)c;
+                        if ((unsigned)c >= p.width || (unsigned)r >= p.height || tx >= lmax.x || ty >= lmax.y) idx = p.last;
+                        D = __ldg(table + idx);
+                        T = T + D;
+                        n++;
+                    } while (__double2hiint(D) != 0 && T <= p.tmax);
+                }
+                range = (T > p.tmax) ? p.tmax : T;
+            } else {
+                // absurd coordinates: the literal reference arithmetic on the layer's geometry and resolution (k_march_lean_het)
+                const double2 r3 = __ldg(rp + 3);
+                const size_t lo = (size_t)((unsigned long long)__double_as_longlong(r3.x) / p.layer_stride_lean * p.layer_stride);
+                const int ti = beam_theta_index(r3.y, i, p.inc, p.theta_dis_f, 1e-6);
+                const double2 sc = __ldg(p.sincos2 + ti);
+                range = march_generic(p.dt + lo, lorig.x, lorig.y, lmax.x, lmax.y, lres.x, __ldg(p.dt + lo + p.last), p.eps_m,
+                                      p.max_range, (int)p.width, r0.x, r0.y, sc.x, sc.y);
+                n = 1;
+            }
+            if (NOISE) {
+                const unsigned long long tick = p.tick_counter ? *p.tick_counter : 0ull;
+                range = range + p.noise_std * normal_sample(p.noise_seed, tick, (uint64_t)a * (uint64_t)p.B + (uint64_t)i);
+            }
+            const double2 r2 = __ldg(rp + 2);
+            if (range <= r2.x) {
+                const double2 cs2 = __ldg(p.cos_side + i);
+                ttc_exact(range, r2.y, cs2.x, cs2.y, p.ttc_thresh, p.ttc_margin, p.wall_flag + a);
+            }
+            p.out[a * (unsigned)p.B + (unsigned)i] = (float)range;      // M * B < 2^32 (host-checked)
+        }
+        if (COUNT) looks += n;
+        const unsigned mx = __reduce_max_sync(0xffffffffu, n);
+        if (lane == 0) mq.cost[it] = mx;
+    }
+    if (COUNT) {
+        const unsigned nsum = __reduce_add_sync(0xffffffffu, looks);
+        if (lane == 0 && nsum) atomicAdd(p.lookup_counter, (unsigned long long)nsum);
+    }
+}
+
 }  // namespace f110

@@ -12,6 +12,8 @@ tensors (N,A,...) that are views of device buffers valid until the next step), n
 scan_noise_std (reference default 0.01; 0 disables the noise for bit-reproducible parity runs).
 Batched mode also takes a list of maps, map=['berlin', 'vegas', ...] with map_ext one extension or a list, stacked into
 one simulator (DeviceMap.stack: one resolution, unrotated origins); env e drives on map env_map_ids[e] (default e % L).
+mixed_resolution=True also stacks maps of different resolutions (e.g. generated tracks with the bundled maps); every map
+of such a batch is then marched in metres, the power-of-two ones included.
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
@@ -55,6 +57,7 @@ class F110Env(object):
                              fov=kwargs.get('fov', 4.7), device=kwargs.get('device', None),
                              noise_std=kwargs.get('scan_noise_std', 0.01))
         self.env_map_ids = kwargs.get('env_map_ids', None)
+        self.mixed_resolution = bool(kwargs.get('mixed_resolution', False))
         self._set_map(self.map_path, self.map_ext)
         self.render_obs = None
         # single-env mode: the whole observation comes back in ONE batch of async copies + one stream sync
@@ -144,10 +147,13 @@ class F110Env(object):
         """Batch extension: re-initialise only the masked envs (counters + Simulator.reset); no tick is run."""
         self.sim.env_reset(poses, env_mask)
 
-    def update_map(self, map_path, map_ext, env_map_ids=None):
-        """f110_env.py:351-362.  Batch extension: lists of map paths (and extensions) as in the constructor."""
+    def update_map(self, map_path, map_ext, env_map_ids=None, mixed_resolution=None):
+        """f110_env.py:351-362.  Batch extension: lists of map paths (and extensions) as in the constructor;
+        env_map_ids / mixed_resolution None keep the current setting."""
         if env_map_ids is not None:
             self.env_map_ids = env_map_ids
+        if mixed_resolution is not None:
+            self.mixed_resolution = bool(mixed_resolution)
         self._set_map(map_path, map_ext)
 
     def _set_map(self, map_path, map_ext):
@@ -171,7 +177,8 @@ class F110Env(object):
                 raise ValueError('env_map_ids must index the list of maps')
             self.sim.set_device_map(layers[0])
         else:
-            self.sim.set_device_map(DeviceMap.stack(layers), env_map_ids=ids)
+            self.sim.set_device_map(DeviceMap.stack(layers, mixed_resolution=self.mixed_resolution),
+                                   env_map_ids=ids)
 
     def update_params(self, params, index=-1):
         """f110_env.py:364-375"""

@@ -86,12 +86,17 @@ class DeviceMap(object):
         return out.contiguous()
 
     @classmethod
-    def stack(cls, maps):
+    def stack(cls, maps, mixed_resolution=False):
         """Multi-map batch (SURVEY 8f row 3): Simulator.set_device_map(stacked, env_map_ids) picks one layer per env.
         Maps that share size, resolution and origin are stacked into one [L][H][W] table.  Other unrotated maps of one
-        resolution are stacked on a canvas (see _stack_canvas); mixed resolutions and rotated origins raise ValueError."""
+        resolution are stacked on a canvas (see _stack_canvas).  Rotated origins raise ValueError, and so do mixed
+        resolutions unless mixed_resolution=True: then the maps are stacked on a metre canvas with each layer's own
+        resolution (see _stack_canvas), and every layer, a power-of-two one included, is marched in metres.  With one
+        shared resolution the flag changes nothing."""
         m0 = maps[0]
         h0 = m0.host
+        if mixed_resolution and any(m.host.resolution != h0.resolution for m in maps[1:]):
+            return cls._stack_canvas(maps, mixed_resolution=True)
         key0 = (h0.height, h0.width, h0.resolution, h0.orig_x, h0.orig_y, h0.orig_c, h0.orig_s)
         if any((m.host.height, m.host.width, m.host.resolution, m.host.orig_x, m.host.orig_y, m.host.orig_c,
                 m.host.orig_s) != key0 for m in maps[1:]):
@@ -116,20 +121,24 @@ class DeviceMap(object):
         return out
 
     @classmethod
-    def _stack_canvas(cls, maps):
+    def _stack_canvas(cls, maps, mixed_resolution=False):
         """Maps of different size and origin on one [L][Hc][Wc] canvas (Wc = max W_l, Hc = max H_l): layer l's table sits in
         the low corner of its slice and every other cell of the slice holds that layer's dt[-1,-1], which is what the
         reference reads off that map, so the march kernels clamp to the canvas and need no per-layer width or height.  The
         cell-unit padded table gets the same treatment with its extra row and column.  f110_map.layer_geom carries each
-        layer's (orig_x, orig_y, x_max = W_l * res, y_max = H_l * res, W_l, H_l)."""
+        layer's (orig_x, orig_y, x_max = W_l * res, y_max = H_l * res, W_l, H_l).
+        mixed_resolution: the layers may differ in resolution.  Only the metre canvas is built (no cell-unit tables,
+        fast_path 0), x_max / y_max are W_l * res_l and H_l * res_l, and f110_map.layer_res carries each layer's
+        (res_l, 1 / res_l) with host copies of the finest and coarsest.  The struct's resolution stays the first map's."""
         hs = [m.host for m in maps]
         h0 = hs[0]
-        if any(h.resolution != h0.resolution for h in hs):
+        if not mixed_resolution and any(h.resolution != h0.resolution for h in hs):
             raise ValueError('stacked maps must share one resolution')
         if any(h.orig_c != 1.0 or h.orig_s != 0.0 for h in hs):
             raise ValueError('stacked maps of different size or origin need unrotated origins')
-        if any((m.dt_cells is None) != (maps[0].dt_cells is None) for m in maps):
+        if not mixed_resolution and any((m.dt_cells is None) != (maps[0].dt_cells is None) for m in maps):
             raise ValueError('stacked maps must all have, or all lack, the cell-unit table')
+        cells = maps[0].dt_cells is not None and not mixed_resolution
         L = len(maps)
         Hc, Wc = max(h.height for h in hs), max(h.width for h in hs)
 
@@ -143,8 +152,8 @@ class DeviceMap(object):
         out.__dict__.update(maps[0].__dict__)
         out.layers = list(maps)
         out.dt = canvas([m.dt for m in maps], 0)
-        out.dt_cells = canvas([m.dt_cells for m in maps], 0) if maps[0].dt_cells is not None else None
-        out.dt_cells_pad = canvas([m.dt_cells for m in maps], 1) if maps[0].dt_cells is not None else None
+        out.dt_cells = canvas([m.dt_cells for m in maps], 0) if cells else None
+        out.dt_cells_pad = canvas([m.dt_cells for m in maps], 1) if cells else None
         out.dt_codes = out.dt_lut = out.dt_codes_pad = None
         out.layer_geom_host = np.array([[h.orig_x, h.orig_y, h.width * h.resolution, h.height * h.resolution, h.width,
                                          h.height] for h in hs], dtype=np.float64)
@@ -162,6 +171,13 @@ class DeviceMap(object):
         c.dt_min_positive = min(m.c.dt_min_positive for m in maps)
         c.layer_geom = nat.ptr(out.layer_geom)
         c.layer_orig_max = float(np.abs(out.layer_geom_host[:, :2]).max())
+        if mixed_resolution:
+            c.fast_path = 0
+            out.layer_res_host = np.array([[h.resolution, 1.0 / h.resolution] for h in hs], dtype=np.float64)
+            out.layer_res = torch.from_numpy(out.layer_res_host).to(maps[0].device)
+            c.layer_res = nat.ptr(out.layer_res)
+            c.layer_res_min = float(out.layer_res_host[:, 0].min())
+            c.layer_res_max = float(out.layer_res_host[:, 0].max())
         out.c = c
         return out
 

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define F110_ABI_VERSION 3
+#define F110_ABI_VERSION 4
 #define F110_NPARAM 18     /* mu C_Sf C_Sr lf lr h m I s_min s_max sv_min sv_max v_switch a_max v_min v_max width length
                               (key order of the default dict, f110_env.py:130) */
 #define F110_NSTATE 7      /* x y steer v yaw yaw_rate slip   (base_classes.py:97) */
@@ -77,10 +77,18 @@ typedef struct {
                                        of a canvas stack, or NULL (every layer has the geometry above).  When set, height / width
                                        are the canvas (max H_l, max W_l); layer l's table sits in the low corner of its canvas
                                        slice and every other cell of the slice (and of the extra row / column of dt_cells_pad)
-                                       holds that layer's dt[-1,-1].  Unrotated origins and one resolution only; needs the lean
-                                       march kernels (F110_ERR_INVALID otherwise) */
+                                       holds that layer's dt[-1,-1].  Unrotated origins and one resolution (or layer_res); needs
+                                       the lean march kernels (F110_ERR_INVALID otherwise) */
     double layer_orig_max;          /* with layer_geom: max over the layers of max(|orig_x|, |orig_y|), a host copy for the
                                        launch-time bound on absurd coordinates (the table itself is device memory) */
+    /* ABI v4 */
+    const double *layer_res;        /* [num_layers][2] (res_l, RN(1/res_l)) of each layer of a canvas stack whose layers differ in
+                                       resolution, or NULL (every layer has `resolution`).  Needs layer_geom (whose x_max / y_max
+                                       are then W_l*res_l, H_l*res_l) and the metre table: fast_path 0, every layer marched in
+                                       metres by the lean canvas-stack kernel; F110_ERR_INVALID on any other path.  Device memory */
+    double layer_res_min, layer_res_max;   /* with layer_res: the finest and coarsest res_l, host copies for the launch-time
+                                       bounds (the 2^31-cell floor and the absurd-coordinate reach use the finest, the
+                                       extents the coarsest) */
 } f110_map;
 
 /* Beam tables RaceCar.__init__ builds once (base_classes.py:122-158) + ScanSimulator2D.__init__ (:360-368). */

@@ -1,13 +1,17 @@
 #!/usr/bin/env python
-"""Multi-track batch benchmark (the `tracks4` workload): one JSON line on stdout.
+"""Multi-track batch benchmark (the `tracks4` and `maps6` workloads): one JSON line on stdout.
 
-    python tools/bench_tracks4.py [--steps 300] [--warmup 30]
+    python tools/bench_tracks4.py [--workload tracks4|maps6] [--steps 300] [--warmup 30]
 
 16384 envs x 2 agents over berlin, vegas, skirk and levine in ONE simulator (a canvas stack, DESIGN.md §2; env e on
 map e % 4; k_march_lean_het), random actions, env level and per-map auto-reset replayed from a CUDA graph as bench.py's
 cfg3.  The same run times each map alone at 16384 x 2 on the single-map path and reports them under `workloads`, so the
 cost of mixing is visible.  Timing, L2 flush and metric follow bench.py (its constants are imported from there).
 Committed line: profiles/h100/bench_tracks4.json.
+
+`--workload maps6`: the same over all six bundled maps (env e on map e % 6), which come in three resolutions (0.05, 0.0504
+and 0.0625 m), so they are stacked with mixed_resolution=True and every layer runs in metres on k_march_lean_het_res;
+example_map alone runs on its cell-unit kernel.  Committed line: profiles/h100/bench_maps6.json.
 """
 import argparse
 import json
@@ -22,6 +26,9 @@ import numpy as np   # noqa: E402
 from bench import FLUSH_BYTES, METRIC, POSE_GAP, SEED, UNIT   # noqa: E402
 
 TRACKS4 = [('berlin', '.png'), ('vegas', '.png'), ('skirk', '.png'), ('levine', '.pgm')]
+MAPS6 = TRACKS4 + [('stata_basement', '.png'), ('example_map', '.png')]
+# workload -> (maps, DeviceMap.stack(mixed_resolution=...))
+WORKLOADS = {'tracks4': (TRACKS4, False), 'maps6': (MAPS6, True)}
 
 
 def gpu_card():
@@ -37,8 +44,8 @@ def gpu_card():
 
 
 def run_tracks4(args):
-    """The multi-track workload: 16384 envs x 2 agents over berlin, vegas, skirk and levine in ONE simulator (canvas stack,
-    env e on map e % 4, k_march_lean_het), random actions, env level and per-map auto-reset in a CUDA graph as cfg3.  Start
+    """The multi-track workload: 16384 envs x 2 agents over the workload's maps in ONE simulator (canvas stack, env e on
+    map e % L; tracks4: berlin, vegas, skirk and levine on k_march_lean_het), random actions, env level and per-map auto-reset in a CUDA graph as cfg3.  Start
     poses come from seeded per-map tables of free-space poses (distance transform >= 0.6 m): only example_map ships a
     raceline.  The same run measures each map alone at 16384 x 2 on the single-map path (`workloads`), which shows what
     mixing costs."""
@@ -47,8 +54,9 @@ def run_tracks4(args):
     dev = torch.device('cuda', 0)
     torch.cuda.set_device(dev)
     K, W = args.steps, args.warmup
-    N, A, B, L = 16384, 2, 1080, len(TRACKS4)
-    maps = [f110.DeviceMap.from_yaml(f110.maps.resolve_map_path(n), e, dev) for n, e in TRACKS4]
+    names, mixed_resolution = WORKLOADS[args.workload]
+    N, A, B, L = 16384, 2, 1080, len(names)
+    maps = [f110.DeviceMap.from_yaml(f110.maps.resolve_map_path(n), e, dev) for n, e in names]
     rng = np.random.default_rng(SEED)
     tables = []
     for m in maps:
@@ -110,14 +118,14 @@ def run_tracks4(args):
                 'kernel_ms': {'k_dynamics': kms[0], 'k_march': kms[1], 'k_tail': kms[2]}, 'launch': record}
 
     ids = np.arange(N) % L
-    main = measure(f110.DeviceMap.stack(maps), ids, dtabs, tables, K, W)
+    main = measure(f110.DeviceMap.stack(maps, mixed_resolution=mixed_resolution), ids, dtabs, tables, K, W)
     singles = {}
-    for l, (name, _) in enumerate(TRACKS4):
+    for l, (name, _) in enumerate(names):
         singles[name] = measure(maps[l], None, dtabs[l], [tables[l]], K, W)
     line = {'metric': METRIC, 'value': main['value'], 'unit': UNIT, 'n_gpus': 1, 'steps': K, 'warmup': W,
             'ms_per_step': main['ms_per_step'], 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
             'dtype': 'f64', 'data': 'synthetic',
-            'config': {'workload': 'tracks4', 'maps': [n for n, _ in TRACKS4], 'env_map_ids': 'e % 4',
+            'config': {'workload': args.workload, 'maps': [n for n, _ in names], 'env_map_ids': 'e %% %d' % L,
                        'num_envs_per_gpu': N, 'num_agents': A, 'num_beams': B, 'integrator': 'RK4', 'timestep': 0.01,
                        'scan_noise': 'off', 'actions': 'steer~U[-0.4189,0.4189], speed~U[0,8] i.i.d. per tick',
                        'auto_reset': 'ego collision -> hashed pose from the map\'s own table of 256 seeded free-space '
@@ -128,11 +136,14 @@ def run_tracks4(args):
             'gpu': gpu_card(), 'step_ms_percentiles': main['step_ms_percentiles'], 'kernel_ms': main['kernel_ms'],
             'launch': main['launch'],
             'workloads': {'%s_alone' % n: r for n, r in singles.items()}}
+    if mixed_resolution:
+        line['config']['mixed_resolution'] = True
     print(json.dumps(line))
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument('--workload', choices=sorted(WORKLOADS), default='tracks4')
     ap.add_argument('--steps', type=int, default=300)
     ap.add_argument('--warmup', type=int, default=30)
     args = ap.parse_args()
