@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, 'libf110_b200.so')
 
 F110_NPARAM = 18
 F110_NSTATE = 7
-ABI_VERSION = 4
+ABI_VERSION = 5
 MAX_START_TABLES = 64
 
 _dp = C.c_void_p   # device / host pointers are passed as raw addresses
@@ -30,7 +30,8 @@ class F110Map(C.Structure):
                 ('dt_cells_pad', _dp), ('dt_codes_pad', _dp), ('codes_pitch', C.c_uint32), ('sincos2', _dp),
                 ('dt_min_positive', C.c_double), ('num_layers', C.c_int32),
                 ('layer_geom', _dp), ('layer_orig_max', C.c_double),
-                ('layer_res', _dp), ('layer_res_min', C.c_double), ('layer_res_max', C.c_double)]
+                ('layer_res', _dp), ('layer_res_min', C.c_double), ('layer_res_max', C.c_double),
+                ('layer_rot', _dp)]
 
 
 class F110Beams(C.Structure):

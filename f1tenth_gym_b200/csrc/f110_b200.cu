@@ -4,10 +4,10 @@
 //   k_dynamics     thread per agent     steer FIFO, pid, RK4/Euler, yaw wrap, scan pose, pose snapshot, the per-agent record of
 //                                       the march (+ extra blocks that sort last tick's work items into the march queue)
 //   k_march_lean   persistent, warp per 32-beam item (march_lean.cuh): LUT heading, sphere tracing on the DT grid, fused iTTC
-//                                       predicate, optional seeded noise, fp32 range out -- the roofline kernel.  Maps with a
-//                                       rotated origin and stand-alone scans run the literal k_raymarch (thread per beam);
-//                                       canvas stacks of maps with different sizes / origins run k_march_lean_het
-//                                       (march_het.cuh)
+//                                       predicate, optional seeded noise, fp32 range out -- the roofline kernel.  Stand-alone
+//                                       scans run the literal k_raymarch (thread per beam); canvas stacks of maps with
+//                                       different sizes / origins run k_march_lean_het (march_het.cuh), maps with a rotated
+//                                       origin, alone or stacked, k_march_lean_rot (march_rot.cuh)
 //   k_tail         warp per agent       GJK vs. the other agents of the env, wall-hit state zeroing, opponent ray-cast inside the
 //                                       blocked-view window, collisions obs, then lap logic and auto-reset per env
 //                                       (k_finalize = the same without the env-level part, for f110_step)
@@ -25,6 +25,7 @@
 #include "march.cuh"
 #include "march_lean.cuh"
 #include "march_het.cuh"
+#include "march_rot.cuh"
 #include "march_tile.cuh"
 #include "planner.cuh"
 #include "edt.cuh"
@@ -201,6 +202,9 @@ struct FirstLookup {
     int agent_queue;                         // 1: the extra blocks build the agent-level queue of the tile march kernel
     const double *__restrict__ layer_geom;   // canvas stack (f110_map.layer_geom): [L][6] per-layer origin and extent, or NULL
     const double *__restrict__ layer_res;    // canvas stack of several resolutions (f110_map.layer_res): [L][2], or NULL
+    const double *__restrict__ layer_rot;    // canvas stack with rotated origins (f110_map.layer_rot): [L][2], or NULL
+    double orig_c, orig_s;                   // one metre map with a rotated origin (rotated = 1)
+    int rotated;
 };
 
 __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__restrict__ actions, double fov,
@@ -254,9 +258,15 @@ __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__re
             k.width = fl.width; k.height = fl.height; k.last = fl.last;
             slot2 = __ldg(fl.cells + lo + cell_index(sx * fl.inv_res, sy * fl.inv_res, k));
         } else {
-            const double tx = sx - g[0], ty = sy - g[1];
+            double tx = sx - g[0], ty = sy - g[1];
             // the layer's own resolution when the layers differ in it (the reference's IEEE division by that map's res)
             const double res = fl.layer_res ? fl.layer_res[2 * (size_t)fl.env_layer[a / s.num_agents]] : fl.res;
+            if (fl.layer_rot) {      // the layer's rotated frame: x_rot, y_rot of xy_2_rc (laser_models.py:75-76)
+                const double *__restrict__ rt = fl.layer_rot + 2 * (size_t)fl.env_layer[a / s.num_agents];
+                const double xr = tx * rt[0] + ty * rt[1];
+                ty = -tx * rt[1] + ty * rt[0];
+                tx = xr;
+            }
             unsigned idx = fl.last;
             if (!(tx < 0 || tx >= g[2] || ty < 0 || ty >= g[3])) {
                 const unsigned c = (unsigned)(int)(tx / res), r = (unsigned)(int)(ty / res);
@@ -268,8 +278,13 @@ __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__re
         CellConsts k;
         k.ox = fl.ox; k.oy = fl.oy; k.eps = 0; k.tmax = 0; k.width = fl.width; k.height = fl.height; k.last = fl.last;
         slot2 = __ldg(fl.cells + lo + cell_index(sx * fl.inv_res, sy * fl.inv_res, k));
-    } else if (fl.cells) {          // literal xy_2_rc (laser_models.py:55-86), unrotated origin
-        const double tx = sx - fl.orig_x, ty = sy - fl.orig_y;
+    } else if (fl.cells) {          // literal xy_2_rc (laser_models.py:55-86)
+        double tx = sx - fl.orig_x, ty = sy - fl.orig_y;
+        if (fl.rotated) {
+            const double xr = tx * fl.orig_c + ty * fl.orig_s;
+            ty = -tx * fl.orig_s + ty * fl.orig_c;
+            tx = xr;
+        }
         unsigned idx = fl.last;
         if (!(tx < 0 || tx >= fl.x_max || ty < 0 || ty >= fl.y_max)) {
             // a quotient that rounds up to width / height is off-map, like every other lookup (lidar.cuh dt_lookup)
@@ -284,8 +299,14 @@ __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__re
     sp[1] = make_double2(slot2, ti0);
     if (fl.rec) {
         // everything the march needs per agent, computed once here instead of once per 32-beam work item
-        // the march takes floor() through the low word of a magic-number add: cell coordinates must stay below 2^31
-        const bool sane = fabs(sx) * fl.inv_res < 1e9 && fabs(sy) * fl.inv_res < 1e9;
+        // the march takes floor() through the low word of a magic-number add: cell coordinates must stay below 2^31.
+        // Unrotated: |x| / res < 1e9 here and, along a ray, |x - orig| / res < 1e9 + reach / res < 1.5e9 (reach: step_impl).
+        // Rotated: |x_rot| <= (|tx| + |ty|)(1 + 2^-51), and along a ray |tx| + |ty| <= |sx| + |sy| + sqrt(2) (max_range +
+        // the largest DT value) + |ox| + |oy| <= |sx| + |sy| + 2 reach, so (|sx| + |sy|) / res < 1e9 and reach < 0.5e9 res
+        // give |x_rot| / res < 2e9 (1 + 2^-50) < 2^31; likewise y_rot.  Anything else takes march_generic_rot, which has the
+        // full row / column checks and needs no bound.
+        const bool sane = (fl.rotated || fl.layer_rot) ? (fabs(sx) + fabs(sy)) * fl.inv_res < 1e9
+                                                       : fabs(sx) * fl.inv_res < 1e9 && fabs(sy) * fl.inv_res < 1e9;
         const bool cells = !fl.metres;
         double2 *rp = fl.rec + 4 * (size_t)a;
         rp[0] = (sane && cells) ? make_double2(sx * fl.inv_res, sy * fl.inv_res) : make_double2(sx, sy);
@@ -1235,6 +1256,23 @@ static void launch_het_res(const LeanK &q, const LayerGeomK &g, const double *la
         launch_het_res_t<1024, 2>(q, g, layer_res, mq, sms * 2u, layers, noise, count, st);
     else launch_het_res_t<512, 4>(q, g, layer_res, mq, sms * 4u, layers, noise, count, st);
 }
+// rotated map origins (march_rot.cuh): one map, or a canvas stack with f110_map.layer_rot; metres, the same block shape rule
+template <int PT, int MINB>
+static void launch_rot_t(const LeanK &q, const RotGeomK &g, const MarchQueue &mq, unsigned blocks, int layers, bool noise,
+                         bool count, cudaStream_t st) {
+    const bool pdl = g_pdl_this_step;
+    snprintf(g_launch_march, sizeof(g_launch_march), "march=lean-rot ROT=1 layers=%d%s CELLS=0 DYN=0 IPT=1 PT=%d MINB=%d NOISE=%d COUNT=%d grid=%u",
+             layers, g.layer_geom ? " HET=1 RES=1" : "", PT, MINB, noise ? 1 : 0, count ? 1 : 0, blocks);
+    if (count) launch_k(k_march_lean_rot<false, true, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, mq);
+    else if (noise) launch_k(k_march_lean_rot<true, false, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, mq);
+    else launch_k(k_march_lean_rot<false, false, PT, MINB>, dim3(blocks), dim3(PT), 0, st, pdl, q, g, mq);
+}
+static void launch_rot(const LeanK &q, const RotGeomK &g, const MarchQueue &mq, unsigned sms, int layers, bool noise, bool count,
+                       cudaStream_t st) {
+    if ((unsigned long long)mq.items >= 700ull * 2ull * (unsigned long long)sms)
+        launch_rot_t<1024, 2>(q, g, mq, sms * 2u, layers, noise, count, st);
+    else launch_rot_t<512, 4>(q, g, mq, sms * 4u, layers, noise, count, st);
+}
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link against libcuda)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
@@ -1387,10 +1425,26 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     // work-item width: march_ipa = ceil(B/32) -> one 32-beam slice per item, ceil(B/64) -> two
     const int item_sub = (sim->march_ipa == (beams->num_beams + 31) / 32) ? 1
                        : (sim->march_ipa == (beams->num_beams + 63) / 64) ? 2 : 0;
-    const bool queued = sim->march_cost && sim->march_order && sim->march_count && variant != 7 &&
-                        item_sub != 0 && sim->march_ipa <= 256 &&
-                        (unsigned long long)NA < (1ull << 22) &&
-                        map->orig_c == 1.0 && map->orig_s == 0.0 && map->sincos && beams->cos_side && variant != 13;
+    // the lean march kernel (march_lean.cuh): 32-beam queue items, `d > eps` == `d != 0` (every positive DT value exceeds
+    // eps), fov < 2 pi (the doubled sin/cos LUT replaces the wrap), LUT indices that fit the Q16.48 fixed point
+    const bool lean_tables = item_sub == 1 && sim->march_rec && map->sincos2 && map->eps >= 0.0 &&
+                             (unsigned long long)NA * (unsigned long long)beams->num_beams < (1ull << 32) &&
+                             (unsigned long long)(map->width + 1) * (unsigned long long)(map->height + 1) < (1ull << 32) &&
+                             map->dt_min_positive > map->eps && beams->fov > 0.0 && beams->fov < 6.283185307179586 &&
+                             beams->theta_index_increment > 0.0 && map->theta_dis < 32768 &&
+                             variant != 1 && variant != 6;
+    const bool queue_tables = sim->march_cost && sim->march_order && sim->march_count && variant != 7 &&
+                              item_sub != 0 && sim->march_ipa <= 256 &&
+                              (unsigned long long)NA < (1ull << 22) && map->sincos && beams->cos_side && variant != 13;
+    // rotated map origins run only on the lean kernel k_march_lean_rot (march_rot.cuh): one metre map that has every table
+    // that kernel needs (any other takes k_raymarch), or a canvas stack with layer_rot (which needs layer_geom and
+    // layer_res, metres only; F110_ERR_INVALID otherwise)
+    const bool het = map->num_layers > 1 && map->layer_geom;
+    if (map->layer_rot && (!het || !map->layer_res || map->fast_path)) return F110_ERR_INVALID;
+    const bool unrotated = map->orig_c == 1.0 && map->orig_s == 0.0;
+    const bool rot_single = !unrotated && !(map->num_layers > 1) && !map->fast_path && queue_tables && lean_tables;
+    const bool rot = rot_single || (het && map->layer_rot);
+    const bool queued = queue_tables && (unrotated || rot);
     const int dyn_blocks = (NA + 127) / 128;
     int order_blocks = queued ? (int)(((long long)NA * sim->march_ipa + 128 * F110_ORDER_ITEMS_PER_THREAD - 1) /
                                          (128 * F110_ORDER_ITEMS_PER_THREAD)) : 0;
@@ -1401,7 +1455,8 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     // (max_range plus one step of at most the map's diagonal) and the origin all stay well inside that bound.  Any other
     // map takes k_raymarch, which has the full row / column checks.
     // (a canvas stack: the largest origin of any layer and the canvas extent, which bounds every layer's)
-    const bool het = map->num_layers > 1 && map->layer_geom;
+    // (a rotated origin: the same bound keeps x_rot / res and y_rot / res below 2^31 for the scan poses k_dynamics passes to
+    // the lean kernel, see `sane` there; march_generic_rot has the full row / column checks)
     // (a canvas stack of several resolutions: the extents at the coarsest layer resolution, the cell bound at the finest;
     // metres only, on the lean canvas-stack kernel)
     if (map->layer_res && (!het || map->fast_path || !(map->layer_res_min > 0.0) || !(map->layer_res_max >= map->layer_res_min)))
@@ -1413,10 +1468,10 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     const double orig_max = het ? fmax(map->layer_orig_max, fmax(fabs(map->orig_x), fabs(map->orig_y)))
                                 : fmax(fabs(map->orig_x), fabs(map->orig_y));
     const double reach = orig_max + 2.0 * (x_ext + y_ext) + map->max_range;
-    const bool cell_march = map->orig_c == 1.0 && map->orig_s == 0.0 && map->sincos && beams->cos_side &&
+    const bool cell_march = (unrotated || rot) && map->sincos && beams->cos_side &&
                             (unsigned long long)map->width * (unsigned long long)map->height < (1ull << 32) &&
                             reach < 0.5 * fmin(1e8, 1e9 * res_fine) && variant != 13;
-    const bool cell_units = cell_march && map->fast_path && map->dt_cells;
+    const bool cell_units = cell_march && !rot && map->fast_path && map->dt_cells;
     FirstLookup fl;
     fl.cells = cell_march ? (cell_units ? map->dt_cells : map->dt) : nullptr;
     fl.metres = cell_units ? 0 : 1;
@@ -1429,14 +1484,7 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     fl.inv_res = 1.0 / res_fine; fl.ox = map->orig_x * fl.inv_res; fl.oy = map->orig_y * fl.inv_res;
     fl.width = (unsigned)map->width; fl.height = (unsigned)map->height;
     fl.last = (unsigned)map->width * (unsigned)map->height - 1u;
-    // the lean march kernel (march_lean.cuh): 32-beam queue items, `d > eps` == `d != 0` (every positive DT value exceeds
-    // eps), fov < 2 pi (the doubled sin/cos LUT replaces the wrap), LUT indices that fit the Q16.48 fixed point
-    const bool lean = queued && cell_march && item_sub == 1 && sim->march_rec && map->sincos2 && map->eps >= 0.0 &&
-                      (!cell_units || map->dt_cells_pad) && (unsigned long long)NA * (unsigned long long)beams->num_beams < (1ull << 32) &&
-                      (unsigned long long)(map->width + 1) * (unsigned long long)(map->height + 1) < (1ull << 32) &&
-                      map->dt_min_positive > map->eps && beams->fov > 0.0 && beams->fov < 6.283185307179586 &&
-                      beams->theta_index_increment > 0.0 && map->theta_dis < 32768 &&
-                      variant != 1 && variant != 6;
+    const bool lean = queued && cell_march && lean_tables && (!cell_units || map->dt_cells_pad);
     // the TMA-tile kernel (march_tile.cuh; variants 30 / 31): single cell-unit map with the padded code table
     const int tile_sz = (variant == 31) ? 160 : 128;
     const bool tile = lean && (variant == 30 || variant == 31) && map->fast_path && map->dt_cells_pad && map->dt_codes_pad &&
@@ -1452,6 +1500,9 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
     if (het && (!lean || tile || !layered)) return F110_ERR_INVALID;
     fl.layer_geom = het ? map->layer_geom : nullptr;
     fl.layer_res = mixres ? map->layer_res : nullptr;
+    fl.layer_rot = het ? map->layer_rot : nullptr;
+    fl.rotated = rot && !het ? 1 : 0;
+    fl.orig_c = map->orig_c; fl.orig_s = map->orig_s;
     k_dynamics<<<dyn_blocks + order_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, dyn_blocks, fl);
     LAUNCH_CHECK("k_dynamics");
     if (ev) CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -1555,6 +1606,14 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
                 t.c_max = (int)map->codes_pitch - tile_sz; t.r_max = map->height + 1 - tile_sz;
                 t.tile_counter = g_tile_counter;
                 if ((rc = launch_tile(t, map, tile_sz, (unsigned)num_sms(), noise, count, st))) return rc;
+            } else if (rot) {
+                RotGeomK g;
+                g.layer_geom = het ? map->layer_geom : nullptr; g.layer_res = het ? map->layer_res : nullptr;
+                g.layer_rot = het ? map->layer_rot : nullptr; g.env_layer = het ? sim->env_layer : nullptr;
+                g.num_agents = (unsigned)sim->num_agents;
+                g.orig = make_double2(map->orig_x, map->orig_y); g.ext = make_double2(mv.x_max, mv.y_max);
+                g.res = make_double2(map->resolution, 1.0 / map->resolution); g.rot = make_double2(map->orig_c, map->orig_s);
+                launch_rot(q, g, mq, (unsigned)num_sms(), map->num_layers, noise, count, st);
             } else if (het) {
                 LayerGeomK g;
                 g.layer_geom = map->layer_geom; g.env_layer = sim->env_layer; g.num_agents = (unsigned)sim->num_agents;
@@ -1664,8 +1723,8 @@ marched:
             if (tail->ar.start_poses) { k_autoreset<<<(sim->num_envs + 127) / 128, 128, 0, st>>>(*sim, tail->ar); LAUNCH_CHECK("k_autoreset"); }
         }
     }
-    snprintf(g_launch_rec, sizeof(g_launch_rec), "%s%s static_runs=%u per_warp=%u %s", g_launch_march, het ? "" : " HET=0",
-             rec_static_runs, rec_per_warp, rec_tail);
+    snprintf(g_launch_rec, sizeof(g_launch_rec), "%s%s%s static_runs=%u per_warp=%u %s", g_launch_march, het ? "" : " HET=0",
+             rot && lean ? "" : " ROT=0", rec_static_runs, rec_per_warp, rec_tail);
     if (ev) CUDA_TRY(cudaEventRecord(ev[3], st));
     return F110_OK;
 }
@@ -1857,7 +1916,7 @@ int f110_scan(const f110_map *map, const f110_beams *beams, const double *poses,
     int rc;
     if ((rc = check_map(map)) || (rc = check_beams(beams))) return rc;
     if (!poses || M <= 0 || (!out_f32 && !out_f64)) return F110_ERR_INVALID;
-    if ((map->num_layers > 1 && map->layer_geom) || map->layer_res) return F110_ERR_INVALID;     // canvas stacks: the tick only
+    if ((map->num_layers > 1 && map->layer_geom) || map->layer_res || map->layer_rot) return F110_ERR_INVALID;     // canvas stacks: the tick only
     MarchArgs g;
     memset(&g, 0, sizeof(g));
     g.scan_pose = poses;

@@ -13,7 +13,8 @@ scan_noise_std (reference default 0.01; 0 disables the noise for bit-reproducibl
 Batched mode also takes a list of maps, map=['berlin', 'vegas', ...] with map_ext one extension or a list, stacked into
 one simulator (DeviceMap.stack: one resolution, unrotated origins); env e drives on map env_map_ids[e] (default e % L).
 mixed_resolution=True also stacks maps of different resolutions (e.g. generated tracks with the bundled maps); every map
-of such a batch is then marched in metres, the power-of-two ones included.
+of such a batch is then marched in metres, the power-of-two ones included.  rotated_origins=True also stacks maps whose
+yaml origin has a yaw (marched in metres in each map's rotated frame by k_march_lean_rot).
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
@@ -58,6 +59,7 @@ class F110Env(object):
                              noise_std=kwargs.get('scan_noise_std', 0.01))
         self.env_map_ids = kwargs.get('env_map_ids', None)
         self.mixed_resolution = bool(kwargs.get('mixed_resolution', False))
+        self.rotated_origins = bool(kwargs.get('rotated_origins', False))
         self._set_map(self.map_path, self.map_ext)
         self.render_obs = None
         # single-env mode: the whole observation comes back in ONE batch of async copies + one stream sync
@@ -147,13 +149,15 @@ class F110Env(object):
         """Batch extension: re-initialise only the masked envs (counters + Simulator.reset); no tick is run."""
         self.sim.env_reset(poses, env_mask)
 
-    def update_map(self, map_path, map_ext, env_map_ids=None, mixed_resolution=None):
+    def update_map(self, map_path, map_ext, env_map_ids=None, mixed_resolution=None, rotated_origins=None):
         """f110_env.py:351-362.  Batch extension: lists of map paths (and extensions) as in the constructor;
-        env_map_ids / mixed_resolution None keep the current setting."""
+        env_map_ids / mixed_resolution / rotated_origins None keep the current setting."""
         if env_map_ids is not None:
             self.env_map_ids = env_map_ids
         if mixed_resolution is not None:
             self.mixed_resolution = bool(mixed_resolution)
+        if rotated_origins is not None:
+            self.rotated_origins = bool(rotated_origins)
         self._set_map(map_path, map_ext)
 
     def _set_map(self, map_path, map_ext):
@@ -177,7 +181,8 @@ class F110Env(object):
                 raise ValueError('env_map_ids must index the list of maps')
             self.sim.set_device_map(layers[0])
         else:
-            self.sim.set_device_map(DeviceMap.stack(layers, mixed_resolution=self.mixed_resolution),
+            self.sim.set_device_map(DeviceMap.stack(layers, mixed_resolution=self.mixed_resolution,
+                                                    rotated_origins=self.rotated_origins),
                                    env_map_ids=ids)
 
     def update_params(self, params, index=-1):

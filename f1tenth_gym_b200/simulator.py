@@ -86,15 +86,22 @@ class DeviceMap(object):
         return out.contiguous()
 
     @classmethod
-    def stack(cls, maps, mixed_resolution=False):
+    def stack(cls, maps, mixed_resolution=False, rotated_origins=False):
         """Multi-map batch (SURVEY 8f row 3): Simulator.set_device_map(stacked, env_map_ids) picks one layer per env.
         Maps that share size, resolution and origin are stacked into one [L][H][W] table.  Other unrotated maps of one
-        resolution are stacked on a canvas (see _stack_canvas).  Rotated origins raise ValueError, and so do mixed
-        resolutions unless mixed_resolution=True: then the maps are stacked on a metre canvas with each layer's own
-        resolution (see _stack_canvas), and every layer, a power-of-two one included, is marched in metres.  With one
-        shared resolution the flag changes nothing."""
+        resolution are stacked on a canvas (see _stack_canvas).  Mixed resolutions raise ValueError unless
+        mixed_resolution=True: then the maps are stacked on a metre canvas with each layer's own resolution (see
+        _stack_canvas), and every layer, a power-of-two one included, is marched in metres.  With one shared resolution
+        the flag changes nothing.
+        Maps whose origin has a yaw raise ValueError unless rotated_origins=True: then the maps are stacked on a metre canvas
+        with each layer's own resolution and rotation (see _stack_canvas), marched by k_march_lean_rot; different
+        resolutions still also need mixed_resolution=True.  Without a rotated map the flag changes nothing."""
         m0 = maps[0]
         h0 = m0.host
+        if len(maps) > 1 and any(m.host.orig_c != 1.0 or m.host.orig_s != 0.0 for m in maps):
+            if not rotated_origins:
+                raise ValueError('stacking maps with a rotated origin needs rotated_origins=True')
+            return cls._stack_canvas(maps, mixed_resolution=mixed_resolution, rotated_origins=True)
         if mixed_resolution and any(m.host.resolution != h0.resolution for m in maps[1:]):
             return cls._stack_canvas(maps, mixed_resolution=True)
         key0 = (h0.height, h0.width, h0.resolution, h0.orig_x, h0.orig_y, h0.orig_c, h0.orig_s)
@@ -121,7 +128,7 @@ class DeviceMap(object):
         return out
 
     @classmethod
-    def _stack_canvas(cls, maps, mixed_resolution=False):
+    def _stack_canvas(cls, maps, mixed_resolution=False, rotated_origins=False):
         """Maps of different size and origin on one [L][Hc][Wc] canvas (Wc = max W_l, Hc = max H_l): layer l's table sits in
         the low corner of its slice and every other cell of the slice holds that layer's dt[-1,-1], which is what the
         reference reads off that map, so the march kernels clamp to the canvas and need no per-layer width or height.  The
@@ -129,16 +136,20 @@ class DeviceMap(object):
         layer's (orig_x, orig_y, x_max = W_l * res, y_max = H_l * res, W_l, H_l).
         mixed_resolution: the layers may differ in resolution.  Only the metre canvas is built (no cell-unit tables,
         fast_path 0), x_max / y_max are W_l * res_l and H_l * res_l, and f110_map.layer_res carries each layer's
-        (res_l, 1 / res_l) with host copies of the finest and coarsest.  The struct's resolution stays the first map's."""
+        (res_l, 1 / res_l) with host copies of the finest and coarsest.  The struct's resolution stays the first map's.
+        rotated_origins: the layers may have rotated origins.  The metre canvas as for mixed_resolution, with layer_res for
+        every layer (also when they share one resolution), and f110_map.layer_rot carries each layer's (orig_c, orig_s)
+        as HostMap computed them.  The struct's origin and rotation stay the first map's."""
         hs = [m.host for m in maps]
         h0 = hs[0]
         if not mixed_resolution and any(h.resolution != h0.resolution for h in hs):
             raise ValueError('stacked maps must share one resolution')
-        if any(h.orig_c != 1.0 or h.orig_s != 0.0 for h in hs):
+        if not rotated_origins and any(h.orig_c != 1.0 or h.orig_s != 0.0 for h in hs):
             raise ValueError('stacked maps of different size or origin need unrotated origins')
-        if not mixed_resolution and any((m.dt_cells is None) != (maps[0].dt_cells is None) for m in maps):
+        metres = mixed_resolution or rotated_origins
+        if not metres and any((m.dt_cells is None) != (maps[0].dt_cells is None) for m in maps):
             raise ValueError('stacked maps must all have, or all lack, the cell-unit table')
-        cells = maps[0].dt_cells is not None and not mixed_resolution
+        cells = maps[0].dt_cells is not None and not metres
         L = len(maps)
         Hc, Wc = max(h.height for h in hs), max(h.width for h in hs)
 
@@ -171,13 +182,17 @@ class DeviceMap(object):
         c.dt_min_positive = min(m.c.dt_min_positive for m in maps)
         c.layer_geom = nat.ptr(out.layer_geom)
         c.layer_orig_max = float(np.abs(out.layer_geom_host[:, :2]).max())
-        if mixed_resolution:
+        if metres:
             c.fast_path = 0
             out.layer_res_host = np.array([[h.resolution, 1.0 / h.resolution] for h in hs], dtype=np.float64)
             out.layer_res = torch.from_numpy(out.layer_res_host).to(maps[0].device)
             c.layer_res = nat.ptr(out.layer_res)
             c.layer_res_min = float(out.layer_res_host[:, 0].min())
             c.layer_res_max = float(out.layer_res_host[:, 0].max())
+        if rotated_origins:
+            out.layer_rot_host = np.array([[h.orig_c, h.orig_s] for h in hs], dtype=np.float64)
+            out.layer_rot = torch.from_numpy(out.layer_rot_host).to(maps[0].device)
+            c.layer_rot = nat.ptr(out.layer_rot)
         out.c = c
         return out
 

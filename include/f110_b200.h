@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define F110_ABI_VERSION 4
+#define F110_ABI_VERSION 5
 #define F110_NPARAM 18     /* mu C_Sf C_Sr lf lr h m I s_min s_max sv_min sv_max v_switch a_max v_min v_max width length
                               (key order of the default dict, f110_env.py:130) */
 #define F110_NSTATE 7      /* x y steer v yaw yaw_rate slip   (base_classes.py:97) */
@@ -77,8 +77,8 @@ typedef struct {
                                        of a canvas stack, or NULL (every layer has the geometry above).  When set, height / width
                                        are the canvas (max H_l, max W_l); layer l's table sits in the low corner of its canvas
                                        slice and every other cell of the slice (and of the extra row / column of dt_cells_pad)
-                                       holds that layer's dt[-1,-1].  Unrotated origins and one resolution (or layer_res); needs
-                                       the lean march kernels (F110_ERR_INVALID otherwise) */
+                                       holds that layer's dt[-1,-1].  Unrotated origins (or layer_rot) and one resolution (or
+                                       layer_res); needs the lean march kernels (F110_ERR_INVALID otherwise) */
     double layer_orig_max;          /* with layer_geom: max over the layers of max(|orig_x|, |orig_y|), a host copy for the
                                        launch-time bound on absurd coordinates (the table itself is device memory) */
     /* ABI v4 */
@@ -89,6 +89,13 @@ typedef struct {
     double layer_res_min, layer_res_max;   /* with layer_res: the finest and coarsest res_l, host copies for the launch-time
                                        bounds (the 2^31-cell floor and the absurd-coordinate reach use the finest, the
                                        extents the coarsest) */
+    /* ABI v5 */
+    const double *layer_rot;        /* [num_layers][2] (orig_c_l, orig_s_l) of each layer of a canvas stack that holds maps with a
+                                       rotated origin, or NULL (every layer unrotated).  Needs layer_geom and layer_res (the rotated
+                                       canvas is metre-only and always carries per-layer resolutions, also when there is only one):
+                                       fast_path 0, every layer marched by k_march_lean_rot; F110_ERR_INVALID without those tables,
+                                       with fast_path or on any other path.  One map with a rotated origin needs no table: its
+                                       orig_c / orig_s above are used.  Device memory */
 } f110_map;
 
 /* Beam tables RaceCar.__init__ builds once (base_classes.py:122-158) + ScanSimulator2D.__init__ (:360-368). */

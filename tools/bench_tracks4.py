@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Multi-track batch benchmark (the `tracks4` and `maps6` workloads): one JSON line on stdout.
+"""Multi-track batch benchmark (the `tracks4`, `maps6` and `rot4` workloads): one JSON line on stdout.
 
-    python tools/bench_tracks4.py [--workload tracks4|maps6] [--steps 300] [--warmup 30]
+    python tools/bench_tracks4.py [--workload tracks4|maps6|rot4] [--steps 300] [--warmup 30]
 
 16384 envs x 2 agents over berlin, vegas, skirk and levine in ONE simulator (a canvas stack, DESIGN.md §2; env e on
 map e % 4; k_march_lean_het), random actions, env level and per-map auto-reset replayed from a CUDA graph as bench.py's
@@ -12,6 +12,12 @@ Committed line: profiles/h100/bench_tracks4.json.
 `--workload maps6`: the same over all six bundled maps (env e on map e % 6), which come in three resolutions (0.05, 0.0504
 and 0.0625 m), so they are stacked with mixed_resolution=True and every layer runs in metres on k_march_lean_het_res;
 example_map alone runs on its cell-unit kernel.  Committed line: profiles/h100/bench_maps6.json.
+
+`--workload rot4`: the four tracks of `tracks4`, each with its yaml origin given a different yaw (ROT4_YAWS), stacked with
+rotated_origins=True on k_march_lean_rot; start tables are built in each map's rotated frame.  Each rotated map alone is
+timed three ways: on k_march_lean_rot (`<map>_alone`), on the literal k_raymarch through debug variant 13
+(`<map>_raymarch_alone`, the path rotated maps took before k_march_lean_rot), and as the unrotated original on its
+default kernel (`<map>_unrotated_alone`).  Committed line: profiles/h100/bench_rot4.json.
 """
 import argparse
 import json
@@ -27,8 +33,10 @@ from bench import FLUSH_BYTES, METRIC, POSE_GAP, SEED, UNIT   # noqa: E402
 
 TRACKS4 = [('berlin', '.png'), ('vegas', '.png'), ('skirk', '.png'), ('levine', '.pgm')]
 MAPS6 = TRACKS4 + [('stata_basement', '.png'), ('example_map', '.png')]
-# workload -> (maps, DeviceMap.stack(mixed_resolution=...))
-WORKLOADS = {'tracks4': (TRACKS4, False), 'maps6': (MAPS6, True)}
+# rot4: the origin yaw of each of the four tracks (rad)
+ROT4_YAWS = [0.35, -0.8, 1.9, 3.0]
+# workload -> (maps, DeviceMap.stack(mixed_resolution=...), origin yaws or None)
+WORKLOADS = {'tracks4': (TRACKS4, False, None), 'maps6': (MAPS6, True, None), 'rot4': (TRACKS4, False, ROT4_YAWS)}
 
 
 def gpu_card():
@@ -54,18 +62,26 @@ def run_tracks4(args):
     dev = torch.device('cuda', 0)
     torch.cuda.set_device(dev)
     K, W = args.steps, args.warmup
-    names, mixed_resolution = WORKLOADS[args.workload]
+    names, mixed_resolution, yaws = WORKLOADS[args.workload]
     N, A, B, L = 16384, 2, 1080, len(names)
-    maps = [f110.DeviceMap.from_yaml(f110.maps.resolve_map_path(n), e, dev) for n, e in names]
-    rng = np.random.default_rng(SEED)
-    tables = []
-    for m in maps:
-        h = m.host
-        free = np.argwhere(h.dt >= 0.6)
-        sel = free[rng.choice(free.shape[0], 256, replace=False)]
-        tables.append(np.stack([(sel[:, 1] + 0.5) * h.resolution + h.orig_x, (sel[:, 0] + 0.5) * h.resolution + h.orig_y,
-                                rng.uniform(0, 2 * np.pi, sel.shape[0])], axis=1))
-    dtabs = [torch.from_numpy(t).to(dev) for t in tables]
+    plain = [f110.DeviceMap.from_yaml(f110.maps.resolve_map_path(n), e, dev) for n, e in names]
+    maps = plain if yaws is None else \
+        [f110.DeviceMap(f110.maps.HostMap(m.host.dt, m.host.resolution, (m.host.orig_x, m.host.orig_y, y)), dev)
+         for m, y in zip(plain, yaws)]
+
+    def start_tables(ms):
+        """256 seeded free-space poses per map, at cell centres of the map's own (rotated) frame, in world coordinates."""
+        rng = np.random.default_rng(SEED)
+        out = []
+        for m in ms:
+            h = m.host
+            free = np.argwhere(h.dt >= 0.6)
+            sel = free[rng.choice(free.shape[0], 256, replace=False)]
+            xr, yr = (sel[:, 1] + 0.5) * h.resolution, (sel[:, 0] + 0.5) * h.resolution
+            out.append(np.stack([h.orig_x + (h.orig_c * xr - h.orig_s * yr), h.orig_y + (h.orig_s * xr + h.orig_c * yr),
+                                 rng.uniform(0, 2 * np.pi, sel.shape[0])], axis=1))
+        return out, [torch.from_numpy(t).to(dev) for t in out]
+    tables, dtabs = start_tables(maps)
     flush = torch.empty(FLUSH_BYTES, dtype=torch.uint8, device=dev)
 
     def measure(dmap, ids, tabs, host_tabs, steps, warmup):
@@ -118,10 +134,21 @@ def run_tracks4(args):
                 'kernel_ms': {'k_dynamics': kms[0], 'k_march': kms[1], 'k_tail': kms[2]}, 'launch': record}
 
     ids = np.arange(N) % L
-    main = measure(f110.DeviceMap.stack(maps, mixed_resolution=mixed_resolution), ids, dtabs, tables, K, W)
+    main = measure(f110.DeviceMap.stack(maps, mixed_resolution=mixed_resolution, rotated_origins=yaws is not None), ids,
+                   dtabs, tables, K, W)
     singles = {}
     for l, (name, _) in enumerate(names):
         singles[name] = measure(maps[l], None, dtabs[l], [tables[l]], K, W)
+    if yaws is not None:
+        lib = f110._native.lib()
+        ptables, pdtabs = start_tables(plain)
+        for l, (name, _) in enumerate(names):
+            lib.f110_debug_set_variant(13)
+            try:
+                singles[name + '_raymarch'] = measure(maps[l], None, dtabs[l], [tables[l]], K, W)
+            finally:
+                lib.f110_debug_set_variant(0)
+            singles[name + '_unrotated'] = measure(plain[l], None, pdtabs[l], [ptables[l]], K, W)
     line = {'metric': METRIC, 'value': main['value'], 'unit': UNIT, 'n_gpus': 1, 'steps': K, 'warmup': W,
             'ms_per_step': main['ms_per_step'], 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
             'dtype': 'f64', 'data': 'synthetic',
@@ -138,6 +165,9 @@ def run_tracks4(args):
             'workloads': {'%s_alone' % n: r for n, r in singles.items()}}
     if mixed_resolution:
         line['config']['mixed_resolution'] = True
+    if yaws is not None:
+        line['config']['rotated_origins'] = True
+        line['config']['origin_yaws'] = dict(zip([n for n, _ in names], yaws))
     print(json.dumps(line))
 
 
