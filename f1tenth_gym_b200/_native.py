@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, 'libf110_b200.so')
 
 F110_NPARAM = 18
 F110_NSTATE = 7
-ABI_VERSION = 5
+ABI_VERSION = 6
 MAX_START_TABLES = 64
 
 _dp = C.c_void_p   # device / host pointers are passed as raw addresses
@@ -82,6 +82,7 @@ SIGNATURES = {
     'f110_step_host_async': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs),
                                        _P(F110HostObs), _dp, _dp, _dp, _dp]),
     'f110_scan': (C.c_int, [_P(F110Map), _P(F110Beams), _dp, C.c_int32, _dp, _dp, _dp, _dp]),
+    'f110_scan_layers': (C.c_int, [_P(F110Map), _P(F110Beams), _dp, _dp, C.c_int32, _dp, _dp, _dp, _dp]),
     'f110_vehicle_dynamics_st': (C.c_int, [_dp, _dp, _dp, C.c_int32, _dp, _dp]),
     'f110_vehicle_dynamics_ks': (C.c_int, [_dp, _dp, _dp, C.c_int32, _dp, _dp]),
     'f110_pid': (C.c_int, [_dp, _dp, C.c_int32, _dp, _dp]),

@@ -7,7 +7,8 @@
 //                                       predicate, optional seeded noise, fp32 range out -- the roofline kernel.  Stand-alone
 //                                       scans run the literal k_raymarch (thread per beam); canvas stacks of maps with
 //                                       different sizes / origins run k_march_lean_het (march_het.cuh), maps with a rotated
-//                                       origin, alone or stacked, k_march_lean_rot (march_rot.cuh)
+//                                       origin, alone or stacked, k_march_lean_rot (march_rot.cuh).  f110_scan_layers runs
+//                                       k_scan_lean (scan_lean.cuh): arbitrary poses, each on its own layer of any map
 //   k_tail         warp per agent       GJK vs. the other agents of the env, wall-hit state zeroing, opponent ray-cast inside the
 //                                       blocked-view window, collisions obs, then lap logic and auto-reset per env
 //                                       (k_finalize = the same without the env-level part, for f110_step)
@@ -26,6 +27,7 @@
 #include "march_lean.cuh"
 #include "march_het.cuh"
 #include "march_rot.cuh"
+#include "scan_lean.cuh"
 #include "march_tile.cuh"
 #include "planner.cuh"
 #include "edt.cuh"
@@ -1925,6 +1927,92 @@ int f110_scan(const f110_map *map, const f110_beams *beams, const double *poses,
     g.lookup_counter = lookup_counter;
     g.total = (long long)M * beams->num_beams;
     return launch_raymarch(make_view(map), make_view(beams), g, map->fast_path != 0, true, (cudaStream_t)stream);
+}
+
+int f110_scan_layers(const f110_map *map, const f110_beams *beams, const double *poses, const int32_t *layer_ids, int32_t M,
+                     float *out_f32, double *out_f64, unsigned long long *lookup_counter, void *stream) {
+    int rc;
+    if ((rc = check_map(map)) || (rc = check_beams(beams))) return rc;
+    if (!poses || M <= 0 || (!out_f32 && !out_f64)) return F110_ERR_INVALID;
+    // the table rules of the tick (step_impl)
+    const bool het = map->num_layers > 1 && map->layer_geom;
+    if (map->layer_rot && (!het || !map->layer_res || map->fast_path)) return F110_ERR_INVALID;
+    if (map->layer_res && (!het || map->fast_path || !(map->layer_res_min > 0.0) || !(map->layer_res_max >= map->layer_res_min)))
+        return F110_ERR_INVALID;
+    const bool unrotated = map->orig_c == 1.0 && map->orig_s == 0.0;
+    if (!unrotated && map->num_layers > 1 && !map->layer_rot) return F110_ERR_INVALID;
+    const unsigned layers = map->num_layers > 1 ? (unsigned)map->num_layers : 1u;
+    if (!layer_ids && layers > 1) return F110_ERR_INVALID;
+    // the lean march's preconditions: `d > eps` == `d != 0`, the doubled LUT instead of the wrap, a Q16.48 LUT index
+    if (!map->sincos2 || !(map->eps >= 0.0) || !(map->dt_min_positive > map->eps) || !(beams->fov > 0.0) ||
+        !(beams->fov < 6.283185307179586) || !(beams->theta_index_increment > 0.0) || map->theta_dis >= 32768)
+        return F110_ERR_INVALID;
+    if ((unsigned long long)M * (unsigned long long)beams->num_beams >= (1ull << 32)) return F110_ERR_INVALID;
+    const int units = (!unrotated || map->layer_rot) ? F110_SCAN_UNITS_ROT
+                    : (map->fast_path && map->dt_cells_pad) ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+    const bool cells = units == F110_SCAN_UNITS_CELLS;
+    const MapView mv = make_view(map);
+    ScanLeanK p;
+    memset(&p, 0, sizeof(p));
+    p.table = cells ? map->dt_cells_pad : map->dt;
+    p.dt = map->dt;
+    p.sincos2 = reinterpret_cast<const double2 *>(map->sincos2);
+    p.poses = poses;
+    p.layer_ids = layers > 1 ? layer_ids : nullptr;
+    p.out_f32 = out_f32; p.out_f64 = out_f64; p.lookup_counter = lookup_counter;
+    p.layer_geom = het ? map->layer_geom : nullptr;
+    p.layer_res = het ? map->layer_res : nullptr;
+    p.layer_rot = het ? map->layer_rot : nullptr;
+    p.orig = make_double2(map->orig_x, map->orig_y); p.ext = make_double2(mv.x_max, mv.y_max);
+    p.res = make_double2(map->resolution, 1.0 / map->resolution); p.rot = make_double2(map->orig_c, map->orig_s);
+    p.tmax = cells ? map->max_range * p.res.y : map->max_range;
+    p.max_range = map->max_range; p.eps = map->eps; p.fov = beams->fov; p.theta_dis_f = (double)map->theta_dis;
+    p.inc = beams->theta_index_increment;
+    p.inc_fx = (unsigned long long)(beams->theta_index_increment * 281474976710656.0 + 0.5);
+    // the guard of the lean tick (step_impl)
+    const double guard = 4.0 * ((double)beams->num_beams * 1.2e-13 + 1e-12);
+    p.guard32 = (unsigned)(guard * 4294967296.0) + 2u;
+    const unsigned long long cells_hw = (unsigned long long)map->width * (unsigned long long)map->height;
+    p.table_stride = cells ? (unsigned long long)(map->width + 1) * (unsigned long long)(map->height + 1) : cells_hw;
+    p.dt_stride = cells_hw;
+    p.width = (unsigned)map->width; p.height = (unsigned)map->height; p.last = (unsigned)(cells_hw - 1ull);
+    p.B = beams->num_beams;
+    p.ipa = (unsigned)((beams->num_beams + 31) / 32);
+    p.items = (unsigned long long)M * p.ipa;
+    p.num_layers = layers;
+    // step_impl's half-bound rule on the origin, the extent and a ray's reach (the finest resolution for the cell bound,
+    // the coarsest for the extents); a map that breaks it, or whose tables do not fit the 32-bit lean indices, takes the
+    // literal path for every pose
+    const bool mixres = het && map->layer_res;
+    const double res_fine = mixres ? map->layer_res_min : map->resolution;
+    const double x_ext = mixres ? map->width * map->layer_res_max : mv.x_max;
+    const double y_ext = mixres ? map->height * map->layer_res_max : mv.y_max;
+    const double orig_max = het ? fmax(map->layer_orig_max, fmax(fabs(map->orig_x), fabs(map->orig_y)))
+                                : fmax(fabs(map->orig_x), fabs(map->orig_y));
+    const double reach = orig_max + 2.0 * (x_ext + y_ext) + map->max_range;
+    p.literal = (reach < 0.5 * fmin(1e8, 1e9 * res_fine) && cells_hw < (1ull << 32) &&
+                 (unsigned long long)(map->width + 1) * (unsigned long long)(map->height + 1) < (1ull << 32)) ? 0 : 1;
+    p.inv_res_fine = 1.0 / res_fine;
+    const unsigned long long blocks = (p.items * 32ull + F110_SCAN_THREADS - 1) / F110_SCAN_THREADS;
+    if (blocks > 0x7fffffffull) return F110_ERR_INVALID;
+    const bool count = lookup_counter != nullptr;
+    static const char *const names[3] = {"cells", "metres", "rot"};
+    snprintf(g_launch_rec, sizeof(g_launch_rec), "scan=lean UNITS=%s layers=%u COUNT=%d LITERAL=%d PT=%d grid=%llu", names[units],
+             layers, count ? 1 : 0, p.literal, F110_SCAN_THREADS, blocks);
+    const cudaStream_t st = (cudaStream_t)stream;
+    const dim3 grid((unsigned)blocks), block(F110_SCAN_THREADS);
+    if (units == F110_SCAN_UNITS_CELLS) {
+        if (count) k_scan_lean<F110_SCAN_UNITS_CELLS, true><<<grid, block, 0, st>>>(p);
+        else k_scan_lean<F110_SCAN_UNITS_CELLS, false><<<grid, block, 0, st>>>(p);
+    } else if (units == F110_SCAN_UNITS_METRES) {
+        if (count) k_scan_lean<F110_SCAN_UNITS_METRES, true><<<grid, block, 0, st>>>(p);
+        else k_scan_lean<F110_SCAN_UNITS_METRES, false><<<grid, block, 0, st>>>(p);
+    } else {
+        if (count) k_scan_lean<F110_SCAN_UNITS_ROT, true><<<grid, block, 0, st>>>(p);
+        else k_scan_lean<F110_SCAN_UNITS_ROT, false><<<grid, block, 0, st>>>(p);
+    }
+    LAUNCH_CHECK("k_scan_lean");
+    return F110_OK;
 }
 
 int f110_vehicle_dynamics_st(const double *x, const double *u, const double *params, int32_t M, double *f, void *stream) {

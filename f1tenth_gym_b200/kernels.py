@@ -113,6 +113,11 @@ def ray_cast(poses, scans, opp_vertices, beams, return_window=False):
     return (s, win) if return_window else s
 
 
+# most beams one f110_scan_layers call writes (M * num_beams < 2^32: the kernel's 32-bit indices); scan(layer_ids=...) splits
+# a larger batch into calls of at most this many beams
+SCAN_LAYERS_MAX_ELEMENTS = (1 << 32) - 1
+
+
 class ScanSimulator2D(object):
     """laser_models.py:348-457.  scan() takes one pose (3,) or a batch (M,3) and returns fp32 ranges
     (M,B) on the device; `rng`/`std_dev` follow the reference: rng=None disables the noise, otherwise
@@ -143,7 +148,11 @@ class ScanSimulator2D(object):
         self.map_resolution = device_map.host.resolution
         return True
 
-    def scan(self, pose, rng=None, std_dev=0.01, out_f64=False, count_lookups=False):
+    def scan(self, pose, rng=None, std_dev=0.01, out_f64=False, count_lookups=False, layer_ids=None):
+        """layer_ids=None: f110_scan on the map (one map; layer 0 of a same-size stack; a canvas stack raises F110Error).
+        layer_ids an int or (M,) ints: f110_scan_layers, pose k on layer layer_ids[k] of the map (any map the Simulator
+        accepts, e.g. set_device_map(sim.map) and layer_ids=sim.env_layer[env_ids]); ValueError for a wrong length or an id
+        outside [0, num_layers)."""
         if self.map_height is None:
             raise ValueError('Map is not set for scan simulator.')
         p = _dev(pose, device=self.device).reshape(-1, 3)
@@ -152,8 +161,18 @@ class ScanSimulator2D(object):
         o64 = torch.empty((M, self.num_beams), dtype=torch.float64, device=self.device) if out_f64 else None
         cnt = torch.zeros((1,), dtype=torch.int64, device=self.device) if count_lookups else None
         L = nat.lib()
-        nat.check(L.f110_scan(C.byref(self.map.c), C.byref(self.beams.c), nat.ptr(p), M, nat.ptr(o32), nat.ptr(o64),
-                              nat.ptr(cnt), _stream_ptr(self.device)))
+        if layer_ids is None:
+            nat.check(L.f110_scan(C.byref(self.map.c), C.byref(self.beams.c), nat.ptr(p), M, nat.ptr(o32), nat.ptr(o64),
+                                  nat.ptr(cnt), _stream_ptr(self.device)))
+        else:
+            ids = self._layer_ids(layer_ids, M)
+            step = max(1, min(SCAN_LAYERS_MAX_ELEMENTS // self.num_beams, 0x7fffffff))
+            for k in range(0, M, step):
+                m = min(step, M - k)
+                nat.check(L.f110_scan_layers(C.byref(self.map.c), C.byref(self.beams.c), nat.ptr(p[k:k + m]),
+                                             nat.ptr(ids[k:k + m]), m, nat.ptr(None if o32 is None else o32[k:k + m]),
+                                             nat.ptr(None if o64 is None else o64[k:k + m]), nat.ptr(cnt),
+                                             _stream_ptr(self.device)))
         out = o64 if out_f64 else o32
         if rng is not None:
             if out_f64:
@@ -162,6 +181,21 @@ class ScanSimulator2D(object):
                                         self._noise_offset, _stream_ptr(self.device)))
             self._noise_offset += out.numel()
         return (out, int(cnt.item())) if count_lookups else out
+
+    def _layer_ids(self, layer_ids, M):
+        """layer_ids (int, or M ints) -> contiguous int32 device tensor [M], checked against the map's layer count."""
+        layers = max(1, int(self.map.c.num_layers))
+        ids = torch.as_tensor(layer_ids) if torch.is_tensor(layer_ids) else torch.as_tensor(np.asarray(layer_ids))
+        if ids.dim() == 0:
+            ids = ids.reshape(1).expand(M)
+        if ids.dim() != 1 or ids.shape[0] != M:
+            raise ValueError('layer_ids must be one int or one per pose (%d), got shape %s' % (M, tuple(ids.shape)))
+        if ids.dtype.is_floating_point or ids.dtype == torch.bool or ids.is_complex():
+            raise ValueError('layer_ids must be integers')
+        lo, hi = int(ids.min()), int(ids.max())
+        if lo < 0 or hi >= layers:
+            raise ValueError('layer_ids must lie in [0, %d), got [%d, %d]' % (layers, lo, hi))
+        return ids.to(device=self.device, dtype=torch.int32).contiguous()
 
     def get_increment(self):
         return self.angle_increment

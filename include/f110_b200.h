@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define F110_ABI_VERSION 5
+#define F110_ABI_VERSION 6
 #define F110_NPARAM 18     /* mu C_Sf C_Sr lf lr h m I s_min s_max sv_min sv_max v_switch a_max v_min v_max width length
                               (key order of the default dict, f110_env.py:130) */
 #define F110_NSTATE 7      /* x y steer v yaw yaw_rate slip   (base_classes.py:97) */
@@ -249,10 +249,25 @@ int f110_pack_scans_u24(const float *scans, int64_t count, uint8_t *out, void *s
 
 /* ScanSimulator2D.scan without noise / get_scan (laser_models.py:148-186, 429-454): M poses -> [M][B].
  * Two deliberate deviations where the reference reads outside its arrays (DESIGN.md §4): a first LUT index of
- * exactly theta_dis reads entry 0, and a cell index that rounds up to width or height reads dt[-1,-1]. */
+ * exactly theta_dis reads entry 0, and a cell index that rounds up to width or height reads dt[-1,-1].
+ * One map only: on a same-size [L][H][W] stack it scans layer 0 for every pose, and a canvas stack (layer_geom,
+ * layer_res or layer_rot) returns F110_ERR_INVALID.  f110_scan_layers scans each pose on a layer of its own, on any map. */
 int f110_scan(const f110_map *map, const f110_beams *beams, const double *poses /* [M][3] */, int32_t M,
               float *out_f32 /* [M][B] or NULL */, double *out_f64 /* [M][B] or NULL */,
               unsigned long long *lookup_counter /* [1] or NULL */, void *stream);
+/* ScanSimulator2D.scan without noise (laser_models.py:148-186, 429-454) for M poses, each on its own layer of `map`.
+ * Batch extension.  poses [M][3] device; layer_ids [M] i32 device, or NULL when the map has one layer.
+ * Accepts every map f110_step accepts: one map (rotated origin or not, any resolution), a same-size [L][H][W] stack, and a
+ * canvas stack in cell units or metres, with layer_res or layer_rot.  Every beam equals the reference's get_scan on that
+ * pose's own map in fp64, with the two deviations of f110_scan; *lookup_counter (optional) gets the reference's lookup
+ * count added.  A layer id outside [0, num_layers) (checked on the device) gives NaN for every beam of its pose and no
+ * lookups.  F110_ERR_INVALID before anything is enqueued: the table rules of f110_step, layer_ids NULL on a map of more
+ * than one layer, sincos2 NULL, dt_min_positive <= eps, fov >= 2 pi, or M * num_beams >= 2^32; F110_ERR_NO_MAP without a
+ * table.  No global state and no host synchronisation: calls on different streams may run at once.  Kernel k_scan_lean
+ * (csrc/scan_lean.cuh), one warp per 32 beams of one pose. */
+int f110_scan_layers(const f110_map *map, const f110_beams *beams, const double *poses, const int32_t *layer_ids, int32_t M,
+                     float *out_f32 /* [M][B] or NULL */, double *out_f64 /* [M][B] or NULL */,
+                     unsigned long long *lookup_counter /* [1] or NULL */, void *stream);
 /* vehicle_dynamics_st (dynamic_models.py:123-176): x [M][7], u [M][2], params [18] -> f [M][7]. */
 int f110_vehicle_dynamics_st(const double *x, const double *u, const double *params, int32_t M, double *f,
                              void *stream);
