@@ -83,6 +83,8 @@ SIGNATURES = {
                                        _P(F110HostObs), _dp, _dp, _dp, _dp]),
     'f110_scan': (C.c_int, [_P(F110Map), _P(F110Beams), _dp, C.c_int32, _dp, _dp, _dp, _dp]),
     'f110_scan_layers': (C.c_int, [_P(F110Map), _P(F110Beams), _dp, _dp, C.c_int32, _dp, _dp, _dp, _dp]),
+    'f110_render_views': (C.c_int, [_P(F110Sim), _P(F110Map), _dp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double,
+                                    C.c_int32, _dp, _dp]),
     'f110_vehicle_dynamics_st': (C.c_int, [_dp, _dp, _dp, C.c_int32, _dp, _dp]),
     'f110_vehicle_dynamics_ks': (C.c_int, [_dp, _dp, _dp, C.c_int32, _dp, _dp]),
     'f110_pid': (C.c_int, [_dp, _dp, C.c_int32, _dp, _dp]),

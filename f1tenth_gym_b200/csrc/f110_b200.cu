@@ -28,6 +28,7 @@
 #include "march_het.cuh"
 #include "march_rot.cuh"
 #include "scan_lean.cuh"
+#include "render.cuh"
 #include "march_tile.cuh"
 #include "planner.cuh"
 #include "edt.cuh"
@@ -2012,6 +2013,55 @@ int f110_scan_layers(const f110_map *map, const f110_beams *beams, const double 
         else k_scan_lean<F110_SCAN_UNITS_ROT, false><<<grid, block, 0, st>>>(p);
     }
     LAUNCH_CHECK("k_scan_lean");
+    return F110_OK;
+}
+
+int f110_render_views(const f110_sim *sim, const f110_map *map, const int32_t *agent_ids, int32_t V, int32_t height,
+                      int32_t width, double metres_per_pixel, double forward_offset, int32_t heading_up, uint8_t *out,
+                      void *stream) {
+    if (!sim || !map || !agent_ids || !out || !sim->state) return F110_ERR_INVALID;
+    if (V < 1 || height < 1 || height > F110_RENDER_MAX_SIZE || width < 1 || width > F110_RENDER_MAX_SIZE) return F110_ERR_INVALID;
+    if (!isfinite(metres_per_pixel) || !(metres_per_pixel > 0.0) || !isfinite(forward_offset)) return F110_ERR_INVALID;
+    if (sim->num_envs <= 0 || sim->num_agents <= 0 || sim->num_agents > F110_RENDER_MAX_AGENTS ||
+        (long long)sim->num_envs * sim->num_agents > 0x7fffffffll)
+        return F110_ERR_INVALID;
+    if (!map->dt || map->height <= 0 || map->width <= 0) return F110_ERR_NO_MAP;
+    if (!(map->resolution > 0.0)) return F110_ERR_INVALID;
+    // the table rules of f110_scan_layers
+    const bool het = map->num_layers > 1 && map->layer_geom;
+    if (map->layer_rot && (!het || !map->layer_res || map->fast_path)) return F110_ERR_INVALID;
+    if (map->layer_res && (!het || map->fast_path || !(map->layer_res_min > 0.0) || !(map->layer_res_max >= map->layer_res_min)))
+        return F110_ERR_INVALID;
+    const bool unrotated = map->orig_c == 1.0 && map->orig_s == 0.0;
+    if (!unrotated && map->num_layers > 1 && !map->layer_rot) return F110_ERR_INVALID;
+    const unsigned layers = map->num_layers > 1 ? (unsigned)map->num_layers : 1u;
+    if (layers > 1 && !sim->env_layer) return F110_ERR_INVALID;
+    RenderK p;
+    memset(&p, 0, sizeof(p));
+    p.state = sim->state;
+    p.env_layer = layers > 1 ? sim->env_layer : nullptr;
+    p.agent_ids = agent_ids;
+    p.dt = map->dt;
+    p.layer_geom = het ? map->layer_geom : nullptr;
+    p.layer_res = het ? map->layer_res : nullptr;
+    p.layer_rot = het ? map->layer_rot : nullptr;
+    p.out = out;
+    p.orig = make_double2(map->orig_x, map->orig_y);
+    p.ext = make_double2(map->width * map->resolution, map->height * map->resolution);    // make_view's x_max / y_max
+    p.rot = make_double2(map->orig_c, map->orig_s);
+    p.res = map->resolution;
+    p.length = sim->sim_length; p.width = sim->sim_width;
+    p.half = metres_per_pixel * 0.5; p.fwd = forward_offset;
+    p.layer_stride = (unsigned long long)map->width * (unsigned long long)map->height;
+    p.map_w = (unsigned)map->width; p.map_h = (unsigned)map->height;
+    p.num_layers = layers;
+    p.NA = sim->num_envs * sim->num_agents; p.A = sim->num_agents;
+    p.V = V; p.H = height; p.W = width; p.heading_up = heading_up ? 1 : 0;
+    const unsigned long long tiles = ((unsigned long long)height * (unsigned long long)width + F110_RENDER_PIXELS - 1) /
+                                     F110_RENDER_PIXELS;
+    const dim3 grid((unsigned)tiles, (unsigned)(V < 65535 ? V : 65535)), block(F110_RENDER_THREADS);
+    k_render_views<<<grid, block, 0, (cudaStream_t)stream>>>(p);
+    LAUNCH_CHECK("k_render_views");
     return F110_OK;
 }
 

@@ -9,7 +9,10 @@ kwargs and defaults are the reference's (f110_env.py:104-159): seed=12345, map='
 params=<18-key dict>, num_agents=2, timestep=0.01, ego_idx=0, integrator=RK4, lidar_dist=0.0.
 Extensions: num_envs (None = single env, reference-shaped numpy/list outputs; int = batched torch
 tensors (N,A,...) that are views of device buffers valid until the next step), num_beams, fov, device,
-scan_noise_std (reference default 0.01; 0 disables the noise for bit-reproducible parity runs).
+scan_noise_std (reference default 0.01; 0 disables the noise for bit-reproducible parity runs),
+local_map={'size': (H, W), 'metres_per_pixel': s, 'forward_offset': f} (adds obs['local_map']: each agent's heading-up class
+view of Simulator.render_views, (N, A, H, W) uint8 on the device in batched mode, numpy (A, H, W) for a single env).
+render(mode='rgb_array') draws each env's ego on the device (world-aligned, the reference window's colours).
 Batched mode also takes a list of maps, map=['berlin', 'vegas', ...] with map_ext one extension or a list, stacked into
 one simulator (DeviceMap.stack: one resolution, unrotated origins); env e drives on map env_map_ids[e] (default e % L).
 mixed_resolution=True also stacks maps of different resolutions (e.g. generated tracks with the bundled maps); every map
@@ -21,11 +24,11 @@ import numpy as np
 import torch
 
 from . import maps as hostmaps
-from .simulator import Integrator, Simulator
+from .simulator import RENDER_MAX_AGENTS, Integrator, Simulator
 
 
 class F110Env(object):
-    metadata = {'render.modes': ['human', 'human_fast']}
+    metadata = {'render.modes': ['human', 'human_fast', 'rgb_array']}
     render_callbacks = []
 
     def __init__(self, **kwargs):
@@ -42,6 +45,9 @@ class F110Env(object):
         self.map_ext = kwargs.get('map_ext', '.png')
         self.params = kwargs.get('params', dict(hostmaps.DEFAULT_PARAMS))
         self.num_agents = kwargs.get('num_agents', 2)
+        self._local_map = self._local_map_settings(kwargs.get('local_map', None))
+        if self._local_map is not None and self.num_agents > RENDER_MAX_AGENTS:
+            raise ValueError('local_map draws at most %d agents per env' % RENDER_MAX_AGENTS)
         self.timestep = kwargs.get('timestep', 0.01)
         self.ego_idx = kwargs.get('ego_idx', 0)
         self.integrator = kwargs.get('integrator', Integrator.RK4)
@@ -62,6 +68,8 @@ class F110Env(object):
         self.rotated_origins = bool(kwargs.get('rotated_origins', False))
         self._set_map(self.map_path, self.map_ext)
         self.render_obs = None
+        self._local_map_buf = None
+        self._palette = None
         # single-env mode: the whole observation comes back in ONE batch of async copies + one stream sync
         # (C ABI f110_step_host) instead of a blocking .cpu() per field
         self._io = None if self.batched else self.sim.make_host_io()
@@ -96,6 +104,8 @@ class F110Env(object):
         sim.env_post_step()
         N, A = self.num_envs, self.num_agents
         if self.batched:
+            if self._local_map is not None:
+                obs['local_map'] = self._render_local_map()
             obs['lap_times'] = sim.lap_times.view(N, A)
             obs['lap_counts'] = sim.lap_counts.view(N, A)
             done = sim.done.bool()
@@ -108,6 +118,8 @@ class F110Env(object):
              'lap_times': sim.lap_times.cpu().numpy(), 'lap_counts': sim.lap_counts.cpu().numpy()}
         for k in ('poses_x', 'poses_y', 'poses_theta', 'linear_vels_x', 'linear_vels_y', 'ang_vels_z'):
             o[k] = [float(v) for v in obs[k][0].cpu().numpy()]
+        if self._local_map is not None:
+            o['local_map'] = self._render_local_map()[0].cpu().numpy()
         done = bool(sim.done[0].item())
         info = {'checkpoint_done': sim.checkpoint_done.bool().cpu().numpy()}
         return o, self.timestep, done, info
@@ -128,6 +140,8 @@ class F110Env(object):
              'linear_vels_y': [0.0] * A, 'ang_vels_z': [float(v) for v in st[5]],
              'collisions': io['collisions'].numpy().copy(),
              'lap_times': io['lap_times'].numpy().copy(), 'lap_counts': lap_counts}
+        if self._local_map is not None:
+            o['local_map'] = self._render_local_map()[0].cpu().numpy()
         # toggle_list >= 4 (f110_env.py:243) <=> lap_counts = floor(toggle / 2) >= 2
         return o, self.timestep, bool(io['done'].numpy()[0]), {'checkpoint_done': lap_counts >= 2}
 
@@ -193,6 +207,56 @@ class F110Env(object):
         """f110_env.py:377-385 (kept for API compatibility; rendering itself is out of scope)."""
         F110Env.render_callbacks.append(callback_func)
 
-    def render(self, mode='human'):
-        assert mode in ['human', 'human_fast']
-        raise NotImplementedError('f1tenth_gym_b200 has no renderer (pyglet/OpenGL GUI is out of scope).')
+    @staticmethod
+    def _local_map_settings(cfg):
+        """local_map kwarg -> (size, metres_per_pixel, forward_offset), or None; ValueError for what render_views refuses."""
+        if cfg is None:
+            return None
+        unknown = set(cfg) - {'size', 'metres_per_pixel', 'forward_offset'}
+        if unknown or 'size' not in cfg or 'metres_per_pixel' not in cfg:
+            raise ValueError("local_map needs 'size' and 'metres_per_pixel' (and optionally 'forward_offset'), got %r" % (cfg,))
+        size = Simulator._view_size(cfg['size'])
+        s, f = float(cfg['metres_per_pixel']), float(cfg.get('forward_offset', 0.0))
+        if not (np.isfinite(s) and s > 0.0) or not np.isfinite(f):
+            raise ValueError('local_map metres_per_pixel must be finite and > 0, forward_offset finite, got %r' % (cfg,))
+        return size, s, f
+
+    def _render_local_map(self):
+        """Every agent's heading-up view into one persistent buffer, (N, A, H, W), overwritten by every step."""
+        (H, W), s, f = self._local_map
+        N, A = self.num_envs, self.num_agents
+        if self._local_map_buf is None:
+            self._local_map_buf = torch.empty((N * A, H, W), dtype=torch.uint8, device=self.sim.device)
+        self.sim.render_views(None, (H, W), s, f, heading_up=True, out=self._local_map_buf)
+        return self._local_map_buf.view(N, A, H, W)
+
+    def render(self, mode='human', env_ids=None, size=(800, 1000), metres_per_pixel=0.024):
+        """mode='rgb_array': each env's ego, world-aligned, as RGB uint8 (Simulator.render_views classes through the reference
+        window's palette, one device gather).  size = (H, W); the defaults are the reference window (1000 x 800 pixels at
+        50 px/m, zoom 1.2).  Batched mode: (K, H, W, 3) CUDA tensor for env_ids (default [0]); single env: numpy (H, W, 3)
+        (env_ids None or [0]).
+        'human' / 'human_fast' (the reference's pyglet window) raise NotImplementedError."""
+        assert mode in self.metadata['render.modes']
+        if mode != 'rgb_array':
+            raise NotImplementedError('f1tenth_gym_b200 has no window renderer (pyglet/OpenGL GUI is out of scope); '
+                                      "use render(mode='rgb_array').")
+        envs = np.arange(1) if env_ids is None else np.asarray(env_ids).reshape(-1)
+        if envs.dtype.kind not in 'iu' or envs.size < 1 or int(envs.min()) < 0 or int(envs.max()) >= self.num_envs:
+            raise ValueError('env_ids must be env indices in [0, %d)' % self.num_envs)
+        if not self.batched and envs.size != 1:
+            raise ValueError('a single env renders one frame: env_ids must be None or [0]')
+        cls = self.sim.render_views(envs * self.num_agents + self.ego_idx, size, metres_per_pixel, 0.0, heading_up=False)
+        if self._palette is None:
+            self._palette = torch.from_numpy(RENDER_PALETTE).to(self.sim.device)
+        # an int32 index (4 bytes per pixel, not the 8 of an int64 one) into the (256, 3) palette
+        rgb = torch.index_select(self._palette, 0, cls.view(-1).to(torch.int32)).view(*cls.shape, 3)
+        return rgb if self.batched else rgb[0].cpu().numpy()
+
+
+# class code -> RGB: the reference window's colours (rendering.py): background for off-map and free, walls, other cars, the
+# followed car; an invalid view (255) is black
+RENDER_PALETTE = np.zeros((256, 3), dtype=np.uint8)
+RENDER_PALETTE[0] = RENDER_PALETTE[1] = (9, 32, 87)
+RENDER_PALETTE[2] = (183, 193, 222)
+RENDER_PALETTE[3] = (99, 52, 94)
+RENDER_PALETTE[4] = (172, 97, 185)

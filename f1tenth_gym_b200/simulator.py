@@ -24,6 +24,10 @@ from . import _native as nat
 from . import maps as hostmaps
 
 
+RENDER_MAX_AGENTS = 64     # csrc/render.cuh F110_RENDER_MAX_AGENTS: car quads a block of k_render_views caches
+RENDER_MAX_SIZE = 8192     # largest view height / width of f110_render_views
+
+
 class Integrator(Enum):     # base_classes.py:40-42
     RK4 = 1
     Euler = 2
@@ -493,6 +497,71 @@ class Simulator(object):
                 'linear_vels_y': self._zeros_NA,
                 'ang_vels_z': st[5].view(N, A),
                 'collisions': self.collisions.view(N, A)}
+
+    # ------------------------------------------------------------------ views
+    def render_views(self, agent_ids=None, size=(64, 64), metres_per_pixel=0.1, forward_offset=0.0, heading_up=True,
+                     out=None):
+        """Top-down class views (C ABI f110_render_views, csrc/render.cuh) -> uint8 (V, H, W) on the device: 0 off-map,
+        1 free, 2 wall (dt == 0), 3 another agent of the env, 4 the followed agent, 255 an invalid view.  View k follows flat
+        agent agent_ids[k] (None: every agent, (N*A, H, W), which reshapes to (N, A, H, W)), centred forward_offset metres
+        ahead of it, with its heading up or world-aligned; size = (H, W) pixels of metres_per_pixel each.
+        Ids given on the host (int, sequence, numpy, CPU tensor) are range-checked (ValueError); a CUDA tensor must be int32
+        (ValueError otherwise) and goes to the kernel unchecked: an id outside [0, N*A) there gives an all-255 view.  With None or a contiguous int32 CUDA
+        tensor of ids and `out` (uint8 CUDA (V, H, W), contiguous) the call is exactly one kernel launch."""
+        H, W = self._view_size(size)
+        s, f = float(metres_per_pixel), float(forward_offset)
+        if not (np.isfinite(s) and s > 0.0):
+            raise ValueError('metres_per_pixel must be finite and > 0, got %r' % (metres_per_pixel,))
+        if not np.isfinite(f):
+            raise ValueError('forward_offset must be finite, got %r' % (forward_offset,))
+        if self.num_agents > RENDER_MAX_AGENTS:
+            raise ValueError('render_views draws at most %d agents per env' % RENDER_MAX_AGENTS)
+        ids = self._view_ids(agent_ids)
+        V = ids.shape[0]
+        if out is None:
+            out = torch.empty((V, H, W), dtype=torch.uint8, device=self.device)
+        elif not (torch.is_tensor(out) and out.dtype == torch.uint8 and out.device == self.state.device and out.is_contiguous()
+                  and tuple(out.shape) == (V, H, W)):
+            # (self.state.device, not self.device: device='cuda' has no index, the tensors allocated on it have one)
+            raise ValueError('out must be a contiguous uint8 tensor of shape %s on %s' % ((V, H, W), self.state.device))
+        nat.check(nat.lib().f110_render_views(C.byref(self.c), C.byref(self._map_struct), nat.ptr(ids), V, H, W, s, f,
+                                              1 if heading_up else 0, nat.ptr(out), _stream_ptr(self.device)))
+        return out
+
+    @staticmethod
+    def _view_size(size):
+        try:
+            H, W = (int(v) for v in size)
+        except (TypeError, ValueError):
+            raise ValueError('size must be (height, width), got %r' % (size,))
+        if tuple(size) != (H, W) or not (1 <= H <= RENDER_MAX_SIZE and 1 <= W <= RENDER_MAX_SIZE):
+            raise ValueError('size must be two ints in [1, %d], got %r' % (RENDER_MAX_SIZE, size))
+        return H, W
+
+    def _view_ids(self, agent_ids):
+        """agent_ids -> contiguous int32 device tensor [V]."""
+        NA = self.num_envs * self.num_agents
+        if agent_ids is None:
+            if getattr(self, '_all_agent_ids', None) is None:
+                self._all_agent_ids = torch.arange(NA, dtype=torch.int32, device=self.device)
+            return self._all_agent_ids
+        if torch.is_tensor(agent_ids) and agent_ids.is_cuda:
+            # passed on as they are, without a host synchronisation: only int32 keeps every id the caller wrote (a narrowing
+            # cast would wrap 2**32 + 3 to agent 3), and the kernel gives an all-255 view for one outside [0, N*A)
+            if agent_ids.dtype != torch.int32:
+                raise ValueError('agent_ids on the device must be int32, got %s' % agent_ids.dtype)
+            ids = agent_ids.reshape(-1)
+        else:
+            a = agent_ids.numpy() if torch.is_tensor(agent_ids) else np.asarray(agent_ids)
+            if a.dtype.kind not in 'iu':
+                raise ValueError('agent_ids must be integers')
+            a = a.reshape(-1)
+            if a.size and (int(a.min()) < 0 or int(a.max()) >= NA):
+                raise ValueError('agent_ids must lie in [0, %d), got [%d, %d]' % (NA, int(a.min()), int(a.max())))
+            ids = torch.from_numpy(a.astype(np.int32))
+        if ids.numel() < 1:
+            raise ValueError('agent_ids must name at least one agent')
+        return ids.to(device=self.device, dtype=torch.int32).contiguous()
 
     # ------------------------------------------------------------------ throughput paths
     def capture_graph(self, actions, autoreset_poses=None, pose_gap=23, autoreset_seed=12345, env_level=False):

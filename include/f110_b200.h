@@ -268,6 +268,21 @@ int f110_scan(const f110_map *map, const f110_beams *beams, const double *poses 
 int f110_scan_layers(const f110_map *map, const f110_beams *beams, const double *poses, const int32_t *layer_ids, int32_t M,
                      float *out_f32 /* [M][B] or NULL */, double *out_f64 /* [M][B] or NULL */,
                      unsigned long long *lookup_counter /* [1] or NULL */, void *stream);
+/* Top-down views of the simulation (batch extension; the reference draws its pyglet window in rendering.py instead): V views
+ * of height x width pixels, row 0 at the top, metres_per_pixel each, view k following agent agent_ids[k] (flat index, i32
+ * device) from its state pose (x, y, yaw), centred forward_offset metres ahead of it, with its heading up (heading_up != 0)
+ * or world-aligned.  out [V][height][width] u8 (device) gets one class per pixel centre: 0 off-map, 1 free, 2 wall (dt == 0,
+ * what the lidar sees), 3 another agent of the env, 4 the followed agent (cars are the get_vertices quads of check_collision,
+ * base_classes.py:549); 255 fills a view whose agent id is outside [0, N*A), whose env layer is outside [0, num_layers) or
+ * whose pose is not finite.  The map class is xy_2_rc (laser_models.py:55-104) on the env's layer, with the deviation of
+ * f110_scan; the exact operation order is in csrc/render.cuh.  Accepts every map f110_step accepts (a stack needs
+ * sim->env_layer).  F110_ERR_INVALID before anything is enqueued: a NULL pointer, V < 1, height or width outside
+ * [1, 8192], metres_per_pixel not finite or <= 0, forward_offset not finite, more than 64 agents per env, a stack without
+ * env_layer or the table rules of f110_scan_layers; F110_ERR_NO_MAP without a table.  Writes nothing but `out`; no global
+ * state, no allocation and no host synchronisation (graph-capturable; calls on two streams may run at once). */
+int f110_render_views(const f110_sim *sim, const f110_map *map, const int32_t *agent_ids, int32_t V, int32_t height,
+                      int32_t width, double metres_per_pixel, double forward_offset, int32_t heading_up, uint8_t *out,
+                      void *stream);
 /* vehicle_dynamics_st (dynamic_models.py:123-176): x [M][7], u [M][2], params [18] -> f [M][7]. */
 int f110_vehicle_dynamics_st(const double *x, const double *u, const double *params, int32_t M, double *f,
                              void *stream);
