@@ -63,6 +63,15 @@ class F110HostObs(C.Structure):
                 ('lap_times', _dp), ('lap_counts', _dp), ('scans_u24', _dp)]
 
 
+class F110Track(C.Structure):
+    _fields_ = [('num_tables', C.c_int32), ('min_segments', C.c_int32), ('table_start', _dp), ('segments', _dp)]
+
+
+class F110Progress(C.Structure):
+    _fields_ = [('seg', _dp), ('s', _dp), ('d', _dp), ('heading_error', _dp), ('progress', _dp), ('delta', _dp),
+                ('back', C.c_int32), ('fwd', C.c_int32), ('reacquire_dist', C.c_double)]
+
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol declared
 # in include/f110_b200.h is exported.
 _P = C.POINTER
@@ -97,6 +106,8 @@ SIGNATURES = {
                                     C.c_double, _dp, _dp]),
     'f110_pure_pursuit_tables': (C.c_int, [_dp, _dp, _dp, _dp, C.c_int32, _dp, _dp, _dp, _dp, C.c_int32, C.c_double,
                                            C.c_double, C.c_double, C.c_double, _dp, _dp]),
+    'f110_track_project': (C.c_int, [_P(F110Track), _dp, _dp, C.c_int32, _dp, _dp]),
+    'f110_track_progress': (C.c_int, [_P(F110Sim), _P(F110Track), _P(F110Progress), _dp]),
     'f110_edt': (C.c_int, [_dp, C.c_int32, C.c_int32, C.c_double, _dp, _dp, _dp, _dp]),
     'f110_rasterize_track': (C.c_int, [_dp, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, _dp, _dp, _dp]),
     'f110_scan_noise': (C.c_int, [_dp, C.c_int64, C.c_double, C.c_uint64, C.c_uint64, _dp]),

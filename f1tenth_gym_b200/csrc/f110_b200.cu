@@ -31,6 +31,7 @@
 #include "render.cuh"
 #include "march_tile.cuh"
 #include "planner.cuh"
+#include "progress.cuh"
 #include "edt.cuh"
 #include "trackgen.cuh"
 
@@ -2153,6 +2154,40 @@ int f110_pure_pursuit_tables(const double *wx, const double *wy, const double *w
         wx, wy, wv, 0, table_start, pose_table, pose_x, pose_y, pose_theta, M, lookahead_distance, vgain, wheelbase,
         max_reacquire, actions_out);
     LAUNCH_CHECK("k_pure_pursuit");
+    return F110_OK;
+}
+
+static bool track_ok(const f110_track *track) {
+    return track && track->num_tables >= 1 && track->min_segments >= 3 && track->table_start && track->segments;
+}
+
+int f110_track_project(const f110_track *track, const double *poses, const int32_t *table_ids, int32_t M, double *out,
+                       void *stream) {
+    if (!track_ok(track) || !poses || !out || M < 1 || (!table_ids && track->num_tables > 1)) return F110_ERR_INVALID;
+    k_track_project<<<(unsigned)(((long long)M * 32 + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+        track->segments, track->table_start, track->num_tables, poses, table_ids, M, out);
+    LAUNCH_CHECK("k_track_project");
+    return F110_OK;
+}
+
+int f110_track_progress(const f110_sim *sim, const f110_track *track, f110_progress *progress, void *stream) {
+    if (!sim || !track_ok(track) || !progress || !sim->state || !sim->steer_cnt) return F110_ERR_INVALID;
+    const f110_progress &g = *progress;
+    if (!g.seg || !g.s || !g.d || !g.heading_error || !g.progress || !g.delta) return F110_ERR_INVALID;
+    if (g.back < 0 || g.fwd < 0 || (long long)g.back + g.fwd + 1 > F110_TRACK_MAX_WINDOW) return F110_ERR_INVALID;
+    if (!isfinite(g.reacquire_dist) || !(g.reacquire_dist > 0.0)) return F110_ERR_INVALID;
+    if (sim->num_envs <= 0 || sim->num_agents <= 0 || (long long)sim->num_envs * sim->num_agents > 0x7fffffffll)
+        return F110_ERR_INVALID;
+    TrackK p;
+    p.state = sim->state; p.steer_cnt = sim->steer_cnt; p.env_layer = sim->env_layer;
+    p.segments = track->segments; p.table_start = track->table_start;
+    p.seg = g.seg; p.s = g.s; p.d = g.d; p.e = g.heading_error; p.progress = g.progress; p.delta = g.delta;
+    p.reacquire_dist = g.reacquire_dist;
+    p.num_tables = track->num_tables;
+    p.NA = sim->num_envs * sim->num_agents; p.A = sim->num_agents;
+    p.back = g.back; p.window = g.back + g.fwd + 1;
+    k_track_progress<<<(unsigned)(((long long)p.NA * 32 + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
+    LAUNCH_CHECK("k_track_progress");
     return F110_OK;
 }
 

@@ -13,6 +13,11 @@ scan_noise_std (reference default 0.01; 0 disables the noise for bit-reproducibl
 local_map={'size': (H, W), 'metres_per_pixel': s, 'forward_offset': f} (adds obs['local_map']: each agent's heading-up class
 view of Simulator.render_views, (N, A, H, W) uint8 on the device in batched mode, numpy (A, H, W) for a single env).
 render(mode='rgb_array') draws each env's ego on the device (world-aligned, the reference window's colours).
+centerline=<(n, 2) table, or one per map of a list> (Simulator.set_centerlines) adds obs['track_s'], obs['track_d'],
+obs['track_heading_error'] and obs['progress'] ((N, A) device tensors in batched mode, numpy (A,) for a single env), updated
+after every step on the device; reward='progress' (needs centerline) returns the ego's progress along its centerline in that
+step, (N,) on the device (a copy, still valid after the next step) or a float, instead of the reference's constant timestep.
+An env reset since its last step restarts its progress at 0, so the step that resets an env earns 0.
 Batched mode also takes a list of maps, map=['berlin', 'vegas', ...] with map_ext one extension or a list, stacked into
 one simulator (DeviceMap.stack: one resolution, unrotated origins); env e drives on map env_map_ids[e] (default e % L).
 mixed_resolution=True also stacks maps of different resolutions (e.g. generated tracks with the bundled maps); every map
@@ -25,6 +30,9 @@ import torch
 
 from . import maps as hostmaps
 from .simulator import RENDER_MAX_AGENTS, Integrator, Simulator
+
+# observation key -> Simulator.update_progress view (added with the centerline kwarg)
+PROGRESS_KEYS = (('track_s', 's'), ('track_d', 'd'), ('track_heading_error', 'heading_error'), ('progress', 'progress'))
 
 
 class F110Env(object):
@@ -66,6 +74,12 @@ class F110Env(object):
         self.env_map_ids = kwargs.get('env_map_ids', None)
         self.mixed_resolution = bool(kwargs.get('mixed_resolution', False))
         self.rotated_origins = bool(kwargs.get('rotated_origins', False))
+        self.reward_kind = kwargs.get('reward', 'timestep')
+        if self.reward_kind not in ('timestep', 'progress'):
+            raise ValueError("reward must be 'timestep' or 'progress', got %r" % (self.reward_kind,))
+        self.centerline = kwargs.get('centerline', None)
+        if self.reward_kind == 'progress' and self.centerline is None:
+            raise ValueError("reward='progress' needs centerline=")
         self._set_map(self.map_path, self.map_ext)
         self.render_obs = None
         self._local_map_buf = None
@@ -103,14 +117,22 @@ class F110Env(object):
         sim = self.sim
         sim.env_post_step()
         N, A = self.num_envs, self.num_agents
+        reward = self.timestep
         if self.batched:
             if self._local_map is not None:
                 obs['local_map'] = self._render_local_map()
             obs['lap_times'] = sim.lap_times.view(N, A)
             obs['lap_counts'] = sim.lap_counts.view(N, A)
+            if self.centerline is not None:
+                p = sim.update_progress()
+                for k, v in PROGRESS_KEYS:
+                    obs[k] = p[v]
+                if self.reward_kind == 'progress':
+                    # a copy: rewards are often kept across steps (rollout buffers), and the delta buffer is overwritten
+                    reward = p['delta'][:, self.ego_idx].clone()
             done = sim.done.bool()
             info = {'checkpoint_done': sim.checkpoint_done.view(N, A).bool()}
-            return obs, self.timestep, done, info
+            return obs, reward, done, info
         # single-env, reference-shaped (base_classes.py:594-612): lists of per-agent values
         o = {'ego_idx': obs['ego_idx'],
              'scans': [s for s in obs['scans'][0].double().cpu().numpy()],
@@ -120,9 +142,19 @@ class F110Env(object):
             o[k] = [float(v) for v in obs[k][0].cpu().numpy()]
         if self._local_map is not None:
             o['local_map'] = self._render_local_map()[0].cpu().numpy()
+        reward = self._progress_single(o)
         done = bool(sim.done[0].item())
         info = {'checkpoint_done': sim.checkpoint_done.bool().cpu().numpy()}
-        return o, self.timestep, done, info
+        return o, reward, done, info
+
+    def _progress_single(self, o):
+        """Single env: the progress keys as numpy (A,) arrays; returns the reward (the ego's delta, or the timestep)."""
+        if self.centerline is None:
+            return self.timestep
+        p = self.sim.update_progress()
+        for k, v in PROGRESS_KEYS:
+            o[k] = p[v][0].cpu().numpy()
+        return float(p['delta'][0, self.ego_idx].item()) if self.reward_kind == 'progress' else self.timestep
 
     def _step_single(self, action):
         """Reference-shaped step of ONE env (base_classes.py:594-612 obs dict of per-agent lists): actions go through a
@@ -142,8 +174,9 @@ class F110Env(object):
              'lap_times': io['lap_times'].numpy().copy(), 'lap_counts': lap_counts}
         if self._local_map is not None:
             o['local_map'] = self._render_local_map()[0].cpu().numpy()
+        reward = self._progress_single(o)
         # toggle_list >= 4 (f110_env.py:243) <=> lap_counts = floor(toggle / 2) >= 2
-        return o, self.timestep, bool(io['done'].numpy()[0]), {'checkpoint_done': lap_counts >= 2}
+        return o, reward, bool(io['done'].numpy()[0]), {'checkpoint_done': lap_counts >= 2}
 
     def step(self, action):
         """f110_env.py:263-304."""
@@ -163,20 +196,31 @@ class F110Env(object):
         """Batch extension: re-initialise only the masked envs (counters + Simulator.reset); no tick is run."""
         self.sim.env_reset(poses, env_mask)
 
-    def update_map(self, map_path, map_ext, env_map_ids=None, mixed_resolution=None, rotated_origins=None):
+    def update_map(self, map_path, map_ext, env_map_ids=None, mixed_resolution=None, rotated_origins=None, centerline=None):
         """f110_env.py:351-362.  Batch extension: lists of map paths (and extensions) as in the constructor;
-        env_map_ids / mixed_resolution / rotated_origins None keep the current setting."""
+        env_map_ids / mixed_resolution / rotated_origins None keep the current setting.  centerline: the new map's table(s) as in
+        the constructor; None turns progress tracking off (the old tables belong to the old map; ValueError with
+        reward='progress')."""
+        if centerline is None and self.reward_kind == 'progress':
+            raise ValueError("reward='progress' needs the new map's centerline=")
         if env_map_ids is not None:
             self.env_map_ids = env_map_ids
         if mixed_resolution is not None:
             self.mixed_resolution = bool(mixed_resolution)
         if rotated_origins is not None:
             self.rotated_origins = bool(rotated_origins)
+        self.centerline = centerline
         self._set_map(map_path, map_ext)
 
     def _set_map(self, map_path, map_ext):
         """One map, or (batched mode) a list of maps stacked into one DeviceMap; env e drives on map env_map_ids[e]
-        (default e % L) and auto-resets from that map's start table when Simulator.tick gets one table per map."""
+        (default e % L) and auto-resets from that map's start table when Simulator.tick gets one table per map.  Then the
+        centerline table(s), if any, for progress tracking."""
+        self._load_map(map_path, map_ext)
+        if self.centerline is not None:
+            self.sim.set_centerlines(self.centerline)
+
+    def _load_map(self, map_path, map_ext):
         if not isinstance(map_path, (list, tuple)):
             self.sim.set_map(map_path, map_ext)
             return

@@ -26,6 +26,7 @@ from . import maps as hostmaps
 
 RENDER_MAX_AGENTS = 64     # csrc/render.cuh F110_RENDER_MAX_AGENTS: car quads a block of k_render_views caches
 RENDER_MAX_SIZE = 8192     # largest view height / width of f110_render_views
+TRACK_MAX_WINDOW = 1024    # csrc/progress.cuh F110_TRACK_MAX_WINDOW: largest back + fwd + 1 of the progress tracker
 
 
 class Integrator(Enum):     # base_classes.py:40-42
@@ -233,6 +234,50 @@ class DeviceBeams(object):
                                nat.ptr(self.cos_side), float(sd.max()))
 
 
+def centerline_segments(table):
+    """One closed centerline (n, 2) (x, y) in metres, progress in row order -> ((n, 8) fp64 segment records, length L).
+    A last row equal to the first is dropped; the table is then closed with segment n-1 -> 0.  Record i = (x_i, y_i, dx, dy,
+    l2 = dx**2 + dy**2, s_i, len_i = sqrt(l2), h_i = arctan2(dy, dx)); s = np.cumsum of the lengths, shifted to start at 0, and
+    L its last entry.  ValueError for fewer than 3 points, non-finite values or a zero-length segment."""
+    T = np.asarray(table.cpu() if torch.is_tensor(table) else table, dtype=np.float64)
+    if T.ndim != 2 or T.shape[1] != 2:
+        raise ValueError('a centerline must be an (n, 2) table of (x, y), got shape %s' % (T.shape,))
+    if not np.all(np.isfinite(T)):
+        raise ValueError('a centerline must hold finite values')
+    if T.shape[0] > 1 and T[-1, 0] == T[0, 0] and T[-1, 1] == T[0, 1]:
+        T = T[:-1]
+    if T.shape[0] < 3:
+        raise ValueError('a centerline needs at least 3 distinct points, got %d' % T.shape[0])
+    d = np.roll(T, -1, axis=0) - T
+    l2 = d[:, 0] ** 2 + d[:, 1] ** 2
+    if np.any(l2 == 0):
+        raise ValueError('a centerline must not repeat a point (zero-length segment %d)' % int(np.argmax(l2 == 0)))
+    length = np.sqrt(l2)
+    cum = np.cumsum(length)
+    s = np.concatenate([[0.0], cum[:-1]])
+    h = np.arctan2(d[:, 1], d[:, 0])
+    return np.ascontiguousarray(np.stack([T[:, 0], T[:, 1], d[:, 0], d[:, 1], l2, s, length, h], axis=1)), float(cum[-1])
+
+
+class CenterlineTables(object):
+    """Closed centerlines on the device (C ABI f110_track): one (n, 2) table, or a list of them (one per map layer)."""
+
+    def __init__(self, tables, device):
+        if isinstance(tables, (list, tuple)) and len(tables) and np.ndim(tables[0]) == 2:
+            tables = list(tables)
+        else:
+            tables = [tables]
+        recs, lengths = zip(*[centerline_segments(t) for t in tables])
+        self.num_tables = len(recs)
+        self.num_segments = [r.shape[0] for r in recs]
+        self.lengths = np.array(lengths, dtype=np.float64)
+        self.records = list(recs)
+        starts = np.concatenate([[0], np.cumsum(self.num_segments)]).astype(np.int32)
+        self.segments = torch.from_numpy(np.concatenate(recs)).to(device)
+        self.table_start = torch.from_numpy(starts).to(device)
+        self.c = nat.F110Track(self.num_tables, min(self.num_segments), nat.ptr(self.table_start), nat.ptr(self.segments))
+
+
 def empty_map_struct():
     """A map struct with no DT bound: stepping with it raises ValueError like the reference
     (laser_models.py:445-446 'Map is not set for scan simulator.')."""
@@ -325,6 +370,9 @@ class Simulator(object):
             nat.ptr(self.march_rec), float(noise_std), int(seed) & 0xFFFFFFFFFFFFFFFF)
         self._graph = None
         self._zeros_NA = torch.zeros((N, A), dtype=torch.float64, device=dev)     # obs['linear_vels_y'] (always 0, :606)
+        self.centerlines = None
+        self.track_seg = self.track_s = self.track_d = self.track_heading_error = None
+        self.track_progress = self.track_delta = None
 
     # ------------------------------------------------------------------ configuration
     def set_map(self, map_path, map_ext, edt='scipy'):
@@ -337,6 +385,7 @@ class Simulator(object):
         self.map = device_map
         self._map_struct = device_map.c
         self._graph = None
+        self.set_centerlines(None)      # the centerlines belong to the old map
         layers = getattr(device_map.c, 'num_layers', 1)
         if layers > 1:
             ids = torch.zeros((self.num_envs,), dtype=torch.int32) if env_map_ids is None else \
@@ -429,6 +478,7 @@ class Simulator(object):
         p = self._poses_tensor(poses)
         m, mp = self._mask_ptr(env_mask)
         nat.check(nat.lib().f110_reset(C.byref(self.c), nat.ptr(p), mp, _stream_ptr(self.device)))
+        self._unacquire(m)
 
     def env_reset(self, poses, env_mask=None):
         """Counters and start frame of F110Env.reset (f110_env.py:319-331) + Simulator.reset."""
@@ -437,6 +487,16 @@ class Simulator(object):
         L = nat.lib()
         nat.check(L.f110_env_reset(C.byref(self.c), nat.ptr(p), mp, _stream_ptr(self.device)))
         nat.check(L.f110_reset(C.byref(self.c), nat.ptr(p), mp, _stream_ptr(self.device)))
+        self._unacquire(m)
+
+    def _unacquire(self, mask):
+        """seg = -1 (not acquired) for the agents of the masked envs (mask: (N,) uint8 device tensor, or None = all)."""
+        if self.track_seg is None:
+            return
+        if mask is None:
+            self.track_seg.fill_(-1)
+        else:
+            self.track_seg.view(self.num_envs, self.num_agents).masked_fill_(mask.bool()[:, None], -1)
 
     def step(self, control_inputs):
         """Simulator.step (base_classes.py:553-612). control_inputs (N,A,2) = (steer, speed)."""
@@ -497,6 +557,85 @@ class Simulator(object):
                 'linear_vels_y': self._zeros_NA,
                 'ang_vels_z': st[5].view(N, A),
                 'collisions': self.collisions.view(N, A)}
+
+    # ------------------------------------------------------------------ centerline progress
+    def set_centerlines(self, tables, window=(8, 56), reacquire_dist=5.0):
+        """Closed centerlines for update_progress / project_centerline (C ABI f110_track, csrc/progress.cuh): one (n, 2) table
+        of (x, y) in metres for a single map, or a list of one table per layer of a stacked map; progress runs in row order.
+        A last row equal to the first is dropped.  window = (back, fwd): a tracked agent searches segments seg - back ..
+        seg + fwd; reacquire_dist: a window whose best distance exceeds it falls back to the global projection.  ValueError for
+        a table of fewer than 3 points, non-finite values, a zero-length segment, a table count other than the map's layer
+        count, back + fwd + 1 outside [1, 1024] or reacquire_dist not finite and > 0.  Every agent starts unacquired.
+        None turns tracking off."""
+        self._graph = None
+        if tables is None:
+            self.centerlines = None
+            self.track_seg = self.track_s = self.track_d = self.track_heading_error = None
+            self.track_progress = self.track_delta = None
+            return
+        try:
+            back, fwd = (int(v) for v in window)
+        except (TypeError, ValueError):
+            raise ValueError('window must be (back, fwd), got %r' % (window,))
+        if back < 0 or fwd < 0 or back + fwd + 1 > TRACK_MAX_WINDOW:
+            raise ValueError('window (back, fwd) needs back, fwd >= 0 and back + fwd + 1 <= %d, got %r'
+                             % (TRACK_MAX_WINDOW, window))
+        r = float(reacquire_dist)
+        if not (np.isfinite(r) and r > 0.0):
+            raise ValueError('reacquire_dist must be finite and > 0, got %r' % (reacquire_dist,))
+        ct = CenterlineTables(tables, self.device)
+        layers = max(1, int(getattr(self._map_struct, 'num_layers', 1)))
+        if ct.num_tables != layers:
+            raise ValueError('%d centerline tables for a map of %d layers' % (ct.num_tables, layers))
+        N, A = self.num_envs, self.num_agents
+        f64 = dict(dtype=torch.float64, device=self.device)
+        self.centerlines = ct
+        self.track_seg = torch.full((N * A,), -1, dtype=torch.int32, device=self.device)
+        self.track_s, self.track_d, self.track_heading_error, self.track_progress, self.track_delta = (
+            torch.zeros((N * A,), **f64) for _ in range(5))
+        self._progress_c = nat.F110Progress(nat.ptr(self.track_seg), nat.ptr(self.track_s), nat.ptr(self.track_d),
+                                            nat.ptr(self.track_heading_error), nat.ptr(self.track_progress),
+                                            nat.ptr(self.track_delta), back, fwd, r)
+        self._progress_views = {'s': self.track_s.view(N, A), 'd': self.track_d.view(N, A),
+                                'heading_error': self.track_heading_error.view(N, A),
+                                'progress': self.track_progress.view(N, A), 'delta': self.track_delta.view(N, A)}
+
+    def _launch_progress(self, L):
+        nat.check(L.f110_track_progress(C.byref(self.c), C.byref(self.centerlines.c), C.byref(self._progress_c),
+                                        _stream_ptr(self.device)))
+
+    def update_progress(self):
+        """One launch (C ABI f110_track_progress): every agent's progress along its map's centerline from the current pose.
+        Returns views (N, A) 's', 'd', 'heading_error', 'progress', 'delta', overwritten by the next update.
+        An agent reset since its last step (reset, env_reset, or the auto-reset of tick) is acquired afresh with progress 0
+        and delta 0.  On the tick that auto-resets an env the update sees the new episode: that tick's delta is 0 and the
+        crash tick's last partial delta is lost."""
+        if self.centerlines is None:
+            raise ValueError('no centerlines: call set_centerlines first')
+        self._launch_progress(nat.lib())
+        return self._progress_views
+
+    def project_centerline(self, poses, table_ids=None):
+        """Stateless projection (C ABI f110_track_project) of poses (M, 3) (x, y, yaw) -> fp64 (M, 5) device tensor of
+        (seg, t, d, s, heading_error); table_ids (M,) ints pick each pose's table (needed with more than one table).  A
+        non-finite pose or a table id outside [0, num_tables) gives a NaN row."""
+        if self.centerlines is None:
+            raise ValueError('no centerlines: call set_centerlines first')
+        p = torch.as_tensor(poses, dtype=torch.float64).to(self.device).reshape(-1, 3).contiguous()
+        M = p.shape[0]
+        if M < 1:
+            raise ValueError('project_centerline needs at least one pose')
+        ids = None
+        if table_ids is not None:
+            ids = torch.as_tensor(table_ids).to(device=self.device, dtype=torch.int32).reshape(-1).contiguous()
+            if ids.numel() != M:
+                raise ValueError('table_ids must hold one table index per pose')
+        elif self.centerlines.num_tables > 1:
+            raise ValueError('%d centerline tables: pass table_ids' % self.centerlines.num_tables)
+        out = torch.empty((M, 5), dtype=torch.float64, device=self.device)
+        nat.check(nat.lib().f110_track_project(C.byref(self.centerlines.c), nat.ptr(p), nat.ptr(ids), M, nat.ptr(out),
+                                               _stream_ptr(self.device)))
+        return out
 
     # ------------------------------------------------------------------ views
     def render_views(self, agent_ids=None, size=(64, 64), metres_per_pixel=0.1, forward_offset=0.0, heading_up=True,
@@ -564,17 +703,22 @@ class Simulator(object):
         return ids.to(device=self.device, dtype=torch.int32).contiguous()
 
     # ------------------------------------------------------------------ throughput paths
-    def capture_graph(self, actions, autoreset_poses=None, pose_gap=23, autoreset_seed=12345, env_level=False):
+    def capture_graph(self, actions, autoreset_poses=None, pose_gap=23, autoreset_seed=12345, env_level=False,
+                      progress=False):
         """Capture one tick (f110_step [+ env_post_step] [+ autoreset]) reading `actions` (a persistent
         device tensor the caller overwrites between replays) into a CUDA graph.  The warm-up tick that precedes the
         capture runs on a snapshot: every simulation buffer (state, FIFO, scans, lap counters, tick counter / noise
-        stream, march queue history) is restored afterwards, so capturing has no side effect on the simulation."""
+        stream, march queue history, progress tracker) is restored afterwards, so capturing has no side effect on the
+        simulation.  progress=True appends update_progress() to the captured tick (needs set_centerlines)."""
         assert actions.is_cuda and actions.dtype == torch.float64 and actions.is_contiguous()
+        if progress and self.centerlines is None:
+            raise ValueError('capture_graph(progress=True) needs set_centerlines first')
         L = nat.lib()
         names = ('state', 'steer_buf', 'steer_cnt', 'scan_pose', 'agent_poses', 'scans', 'wall_flag', 'collisions',
                  'collision_idx', 'current_time', 'lap_times', 'lap_counts', 'toggle_list', 'near_starts', 'start_xs',
                  'start_ys', 'start_thetas', 'start_rot', 'done', 'checkpoint_done', 'tick_counter', 'march_cost',
-                 'march_order', 'march_count', 'march_rec')
+                 'march_order', 'march_count', 'march_rec', 'track_seg', 'track_s', 'track_d', 'track_heading_error',
+                 'track_progress', 'track_delta')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
 
@@ -582,6 +726,8 @@ class Simulator(object):
             nat.check(L.f110_tick(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c), nat.ptr(actions),
                                   1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(autoreset_seed),
                                   _stream_ptr(self.device)))
+            if progress:
+                self._launch_progress(L)
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
@@ -595,7 +741,7 @@ class Simulator(object):
         with torch.cuda.graph(g):
             tick()
         self._graph = g
-        self._graph_keep = (actions, table)
+        self._graph_keep = (actions, table) + ((self.centerlines, self._progress_views) if progress else ())
         return g
 
     def replay(self):

@@ -325,6 +325,53 @@ int f110_pure_pursuit_tables(const double *wx, const double *wy, const double *w
                              const double *pose_theta, int32_t M, double lookahead_distance, double vgain, double wheelbase,
                              double max_reacquire, double *actions_out, void *stream);
 
+/* ---- centerline progress (batch extension: the reference's reward is the constant timestep, f110_env.py:263-304) ---- */
+
+/* Closed centerlines, one table per map layer.  Table t holds segments [table_start[t], table_start[t+1]) of `segments`; segment
+ * i of a table of n points runs from point i to point (i + 1) mod n, and its record is 8 fp64 values (x_i, y_i, dx, dy, l2,
+ * s_i, len_i, h_i): dx, dy = next point - point, l2 = dx*dx + dy*dy, len_i = sqrt(l2), s_i = arc length at point i
+ * (np.cumsum of len, 0 for point 0), h_i = atan2(dy, dx).  A table's length L is s_{n-1} + len_{n-1}. */
+typedef struct {
+    int32_t num_tables;
+    int32_t min_segments;           /* host copy: the fewest segments of any table (>= 3) */
+    const int32_t *table_start;     /* [num_tables + 1] i32, device */
+    const double *segments;         /* [table_start[num_tables]][8] fp64, device */
+} f110_track;
+
+/* Per-agent tracker state and outputs, [N*A] device buffers each (flat agent index). */
+typedef struct {
+    int32_t *seg;                   /* state: segment of the last projection, -1 = not acquired */
+    double *s;                      /* arc length of the last projection (also the previous s of the next update) */
+    double *d;                      /* signed lateral offset, positive left of the direction of travel */
+    double *heading_error;          /* yaw - h_i wrapped to [-pi, pi) */
+    double *progress;               /* arc length travelled since the agent was acquired */
+    double *delta;                  /* progress made by the last update */
+    int32_t back, fwd;              /* the tracking window: segments seg - back .. seg + fwd (1 <= back + fwd + 1 <= 1024) */
+    double reacquire_dist;          /* a window whose best distance exceeds this falls back to the global projection */
+} f110_progress;
+
+/* nearest_point_on_trajectory (reference examples/waypoint_follow.py:16-47) on the closed table vstack(T, T[0]) in its operation
+ * order, fp64, the first minimum by segment index; its np.dot is BLAS ddot, dot = fma(py - y, dy, (px - x) * dx), and no other
+ * operation is fused (csrc/progress.cuh): poses [M][3] (x, y, yaw, device), table_ids [M] i32 (device), or
+ * NULL with a single table -> out [M][5] = (seg, t, d, s, e): segment, t in [0, 1], signed distance (+ left of travel),
+ * s = s_i + t * len_i, heading error yaw - h_i wrapped by e - 2pi * floor((e + pi) / 2pi).  A non-finite pose or a table id
+ * outside [0, num_tables) gives a NaN row.  F110_ERR_INVALID before anything is enqueued: NULL pointers, M < 1, no table,
+ * min_segments < 3, table_ids NULL with more than one table.  No global state, allocation or host synchronisation. */
+int f110_track_project(const f110_track *track, const double *poses, const int32_t *table_ids, int32_t M, double *out,
+                       void *stream);
+
+/* One update of every agent's progress along its map's centerline (table env_layer[env], or table 0 when sim->env_layer is
+ * NULL), from the pose in sim->state.  Acquire when seg < 0 or sim->steer_cnt == 0 (the agent was reset since its last step:
+ * f110_reset and the auto-reset zero it, every step increments it): the projection of f110_track_project, progress = delta = 0.
+ * Otherwise track: the first minimum over the window k = 0 .. back + fwd, segment (seg - back + k) mod n, in window order
+ * (clipped to n segments); a best distance above reacquire_dist falls back to the global projection and keeps the progress;
+ * delta = s - s_prev, minus L if above L/2, plus L if below -L/2, and progress += delta.  On the tick that auto-resets an env
+ * the update already sees the new episode, so that tick's delta is 0 and the crash tick's last partial delta is lost.
+ * A non-finite pose or a bad table id gives NaN outputs and seg = -1.  F110_ERR_INVALID before anything is enqueued: NULL
+ * pointers, no table, min_segments < 3, a bad window, reacquire_dist not finite or <= 0.  No global state, allocation or
+ * host synchronisation: capturable in a CUDA graph after f110_tick.  Kernel k_track_progress (csrc/progress.cuh). */
+int f110_track_progress(const f110_sim *sim, const f110_track *track, f110_progress *progress, void *stream);
+
 /* Exact Euclidean distance transform on the device (load-time; reference laser_models.py:40-53 get_dt =
  * resolution * scipy.ndimage.distance_transform_edt(bitmap)): occupied [H][W] u8 (1 where the thresholded image
  * is 0), scratch [H][W] i32, dt_out [H][W] f64 = resolution * sqrt(k) with k the exact squared cell distance
