@@ -34,6 +34,10 @@ class F110Map(C.Structure):
                 ('layer_rot', _dp)]
 
 
+class F110MarchTables(C.Structure):
+    _fields_ = [('dt_cells_brick', _dp)]
+
+
 class F110Beams(C.Structure):
     _fields_ = [('num_beams', C.c_int32),
                 ('fov', C.c_double), ('angle_increment', C.c_double), ('theta_index_increment', C.c_double),
@@ -81,15 +85,24 @@ SIGNATURES = {
     'f110_last_cuda_error': (C.c_char_p, []),
     'f110_step': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp]),
     'f110_step_profile': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _P(C.c_float), _dp]),
+    'f110_step_ex': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, _dp]),
+    'f110_step_profile_ex': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, _P(C.c_float),
+                                       _dp]),
+    'f110_map_brick_elems': (C.c_int64, [_P(F110Map)]),
+    'f110_map_brick': (C.c_int, [_P(F110Map), _dp, _dp]),
     'f110_reset': (C.c_int, [_P(F110Sim), _dp, _dp, _dp]),
     'f110_env_reset': (C.c_int, [_P(F110Sim), _dp, _dp, _dp]),
     'f110_env_post_step': (C.c_int, [_P(F110Sim), _dp]),
     'f110_autoreset': (C.c_int, [_P(F110Sim), _dp, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _dp]),
     'f110_tick': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, C.c_int32, _dp, C.c_int32, C.c_int32,
                             C.c_uint64, _dp]),
+    'f110_tick_ex': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32, _dp, C.c_int32,
+                               C.c_int32, C.c_uint64, _dp]),
     'f110_step_host': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs), _dp]),
     'f110_step_host_async': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs),
                                        _P(F110HostObs), _dp, _dp, _dp, _dp]),
+    'f110_step_host_async_ex': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, _dp,
+                                          _P(F110HostObs), _P(F110HostObs), _dp, _dp, _dp, _dp]),
     'f110_scan': (C.c_int, [_P(F110Map), _P(F110Beams), _dp, C.c_int32, _dp, _dp, _dp, _dp]),
     'f110_scan_layers': (C.c_int, [_P(F110Map), _P(F110Beams), _dp, _dp, C.c_int32, _dp, _dp, _dp, _dp]),
     'f110_render_views': (C.c_int, [_P(F110Sim), _P(F110Map), _dp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double,

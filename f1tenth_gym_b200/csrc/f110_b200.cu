@@ -1042,8 +1042,10 @@ static int num_sms() {
 // fp64 table, half of the queue dynamic); 66 / 60 / 61 = static dealing with 4 x 512 / 2 x 1024 / 8 x 256 threads per SM;
 // 40 / 41 / 42 = dynamic with 4 x 512 / 3 x 512 / 2 x 1024; 20 / 22 = rank-coded table + shared LUT; 21 = 48 warps/SM;
 // 30 / 31 = TMA tile 128 / 160 cells; 62-65 = thread-block clusters sharing a ticket counter; 1 / 6 = round-1 persistent kernel
-// (fp64 / coded); 7 / 9 = no queue (block per 64-beam tile); 13 = the literal k_raymarch
+// (fp64 / coded); 7 / 9 = no queue (block per 64-beam tile); 13 = the literal k_raymarch; 90 = variant 0 on the padded
+// row-major table even when a brick table is bound (f110_march_tables)
 static int g_variant = -1, g_chunk = -1;
+static bool g_no_brick = false;        // variant 90
 // Dynamic second half of the queue (k_march_lean<DYN>): every block gets g_dyn_pct % of its fair share dealt statically and claims
 // the rest in runs from one global counter, g_dyn_ahead runs ahead of their use.  50 % / 4 was the measured optimum at cfg3, cfg2x2
 // and cfg2: the default of variant 0.
@@ -1053,8 +1055,18 @@ static int rm_variant() {
     if (g_variant < 0) {
         const char *e = getenv("F110_MARCH_VARIANT");
         g_variant = e ? atoi(e) : 0;
+        if (g_variant == 90) { g_variant = 0; g_no_brick = true; }
     }
     return g_variant;
+}
+
+// the brick table of a map (f110_map_brick, k_march_lean_brick): 4 x 4-cell bricks over the (height + 1) x (width + 1) padded
+// table, bricks per row and elements (0 when the element index would not fit 32 bits)
+#define F110_BRICK_MAX_BEAMS 1080
+static unsigned long long brick_cols(const f110_map *map) { return ((unsigned long long)map->width + 4ull) / 4ull; }
+static unsigned long long brick_elems(const f110_map *map) {
+    const unsigned long long n = brick_cols(map) * 16ull * (((unsigned long long)map->height + 4ull) / 4ull);
+    return n < (1ull << 32) ? n : 0ull;
 }
 
 static int launch_raymarch(const MapView &mv, const BeamView &bv, const MarchArgs &g, bool fast, bool standalone,
@@ -1149,6 +1161,24 @@ static void launch_lean_t(const LeanK &q, const MarchQueue &mq, unsigned blocks,
     else if (noise) launch_k(k_march_lean<TABLE, true, false, CELLS, LAYERED, PT, MINB, DYN, 1, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
     else launch_k(k_march_lean<TABLE, false, false, CELLS, LAYERED, PT, MINB, DYN, 1, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
 }
+// k_march_lean_brick: the launches of the single cell-unit map (launch_lean, variant 0) on the brick table
+template <int PT, int MINB, bool DYN, int IPT, int RING>
+static void launch_brick_t(const LeanK &q, const MarchQueue &mq, unsigned blocks, bool noise, bool count, cudaStream_t st) {
+    const bool pdl = g_pdl_this_step;
+    snprintf(g_launch_march, sizeof(g_launch_march),
+             "march=lean TABLE=0 CELLS=1 LAYERED=0 DYN=%d IPT=%d RING=%d PT=%d MINB=%d NOISE=%d COUNT=%d grid=%u layout=brick4x4",
+             DYN ? 1 : 0, IPT, RING, PT, MINB, noise ? 1 : 0, count ? 1 : 0, blocks);
+    if (count) launch_k(k_march_lean_brick<false, true, PT, MINB, DYN, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
+    else if (noise) launch_k(k_march_lean_brick<true, false, PT, MINB, DYN, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
+    else launch_k(k_march_lean_brick<false, false, PT, MINB, DYN, IPT, RING>, dim3(blocks), dim3(PT), 0, st, pdl, q, mq);
+}
+static void launch_brick(const LeanK &q, const MarchQueue &mq, unsigned sms, bool noise, bool count, bool dyn, cudaStream_t st) {
+    if (!dyn) launch_brick_t<512, 4, false, 1, 0>(q, mq, sms * 4u, noise, count, st);
+    else if (mq.uniform_ipt4 == 4u) launch_brick_t<512, 4, true, 4, 2>(q, mq, sms * 4u, noise, count, st);
+    else if (mq.uniform_ipt4 == 2u) launch_brick_t<512, 4, true, 2, 2>(q, mq, sms * 4u, noise, count, st);
+    else launch_brick_t<512, 4, true, 0, 2>(q, mq, sms * 4u, noise, count, st);
+}
+
 static void launch_lean(const LeanK &q, const MarchQueue &mq, unsigned sms, bool cells, bool coded, bool occ3, bool layered,
                         bool noise, bool count, bool dyn, cudaStream_t st) {
     // thread-block clusters sharing one ticket counter (variants 62-65), plain noise-free marching only
@@ -1357,7 +1387,10 @@ int f110_abi_version(void) { return F110_ABI_VERSION; }
  * (smid, start ns, end ns, max steps of warp 0) per block; NULL switches it off. */
 void f110_debug_set_trace(unsigned long long *buf) { g_trace = buf; }
 /* measurement aid (not in the public header): select the march kernel variant at run time (tools/ab_march.py) */
-void f110_debug_set_variant(int variant) { g_variant = variant < 0 ? 0 : variant; }
+void f110_debug_set_variant(int variant) {
+    g_no_brick = variant == 90;
+    g_variant = (variant < 0 || variant == 90) ? 0 : variant;
+}
 void f110_debug_set_dyn(int static_pct, int ahead) {
     g_dyn_pct = static_pct < 0 ? 0 : (static_pct > 100 ? 100 : static_pct);
     g_dyn_ahead = ahead < 1 ? 1 : (ahead > 8 ? 8 : ahead);
@@ -1407,8 +1440,8 @@ struct TailOpts {
     AutoResetArgs ar;
 };
 
-static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
-                     cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail = nullptr) {
+static int step_impl(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                     const double *actions, cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail = nullptr) {
     int rc;
     if ((rc = check_sim(sim)) || (rc = check_map(map)) || (rc = check_beams(beams))) return rc;
     if (!actions) return F110_ERR_INVALID;
@@ -1594,13 +1627,23 @@ static int step_impl(const f110_sim *sim, const f110_map *map, const f110_beams 
             q.guard32 = (unsigned)(guard * 4294967296.0) + 2u;
             q.width = k.width; q.height = k.height; q.last = k.last; q.B = k.B;
             q.layer_stride = fl.layer_stride; q.layer_stride_lean = fl.rec_layer_stride;
-            q.dt = map->dt; q.orig_x = map->orig_x; q.orig_y = map->orig_y; q.dt_oob_unused = 0.0; q.eps_m = map->eps;
+            q.dt = map->dt; q.orig_x = map->orig_x; q.orig_y = map->orig_y; q.brick_cols1 = 0u; q.unused = 0u; q.eps_m = map->eps;
             q.max_range = map->max_range;
             q.codes_pitch = map->codes_pitch;
             const bool lcoded = cell_units && !layered && map->dt_codes_pad && map->dt_lut && map->codes_pitch > (unsigned)map->width &&
                                 (variant == 20 || variant == 22);
             const bool occ3 = (variant == 21 || variant == 22 || variant == 41);
-            if (tile) {
+            // the brick table (f110_march_tables): a single fp64 cell-unit map on the default launch, up to 1080 beams per scan.
+            // Measured (H100, bench.py, against the row-major table): 5-8 % off the march at 270-1080 beams, 4 % slower at 2160,
+            // where a warp's rays are close enough together that the row-major gathers already touch few lines
+            const bool brick = tables && tables->dt_cells_brick && cell_units && !layered && !(map->num_layers > 1) && !het &&
+                               !lcoded && !tile && variant == 0 && !g_no_brick && beams->num_beams <= F110_BRICK_MAX_BEAMS &&
+                               brick_elems(map) != 0ull;
+            q.brick_cols1 = brick ? (unsigned)(brick_cols(map) - 1ull) : 0u;
+            if (brick) {
+                q.table = tables->dt_cells_brick;
+                launch_brick(q, mq, (unsigned)num_sms(), noise, count, mq.static_runs >= mq.dyn_ahead, st);
+            } else if (tile) {
                 TileK t;
                 t.l = q;
                 t.order = sim->march_order; t.count = sim->march_count; t.claim = sim->march_count + 3;
@@ -1735,15 +1778,23 @@ marched:
 
 int f110_step(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
               void *stream) {
-    return step_impl(sim, map, beams, actions, (cudaStream_t)stream, nullptr);
+    return f110_step_ex(sim, map, nullptr, beams, actions, stream);
+}
+int f110_step_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                 const double *actions, void *stream) {
+    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr);
 }
 
 int f110_step_profile(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
                       float *kernel_ms /* host [3] */, void *stream) {
+    return f110_step_profile_ex(sim, map, nullptr, beams, actions, kernel_ms, stream);
+}
+int f110_step_profile_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                         const double *actions, float *kernel_ms /* host [3] */, void *stream) {
     if (!kernel_ms) return F110_ERR_INVALID;
     cudaEvent_t ev[4];
     for (int i = 0; i < 4; i++) CUDA_TRY(cudaEventCreate(&ev[i]));
-    int rc = step_impl(sim, map, beams, actions, (cudaStream_t)stream, ev);
+    int rc = step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, ev);
     if (rc == F110_OK) {
         cudaError_t e = cudaEventSynchronize(ev[3]);
         if (e != cudaSuccess) rc = cuda_fail(e, "cudaEventSynchronize");
@@ -1824,6 +1875,11 @@ int f110_autoreset(const f110_sim *sim, const double *start_poses, int32_t num_s
 int f110_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
               int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
               void *stream) {
+    return f110_tick_ex(sim, map, nullptr, beams, actions, env_level, start_poses, num_start, pose_gap, seed, stream);
+}
+int f110_tick_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                 const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                 uint64_t seed, void *stream) {
     int rc;
     if ((rc = check_sim(sim))) return rc;
     if (env_level && (rc = check_env_arrays(sim))) return rc;
@@ -1835,7 +1891,7 @@ int f110_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams,
     t.ar.num_tables = 0;
     if (start_poses && (rc = start_tables(sim, num_start, t.ar))) return rc;
     if (t.ar.num_tables && (!map || t.ar.num_tables != map->num_layers)) return F110_ERR_INVALID;
-    return step_impl(sim, map, beams, actions, (cudaStream_t)stream, nullptr, &t);
+    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, &t);
 }
 
 int f110_step_host(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions_host,
@@ -1851,7 +1907,7 @@ int f110_step_host(const f110_sim *sim, const f110_map *map, const f110_beams *b
     TailOpts t;
     t.fused = true; t.env_level = env_level ? 1 : 0;
     t.ar.start_poses = nullptr; t.ar.num_start = 0; t.ar.pose_gap = 0; t.ar.seed = 0; t.ar.tick_host = 0;
-    if ((rc = step_impl(sim, map, beams, actions_dev_scratch, st, nullptr, &t))) return rc;
+    if ((rc = step_impl(sim, map, nullptr, beams, actions_dev_scratch, st, nullptr, &t))) return rc;
     if (out->scans)
         CUDA_TRY(cudaMemcpyAsync(out->scans, sim->scans, NA * beams->num_beams * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (out->state)
@@ -1874,6 +1930,13 @@ int f110_step_host_async(const f110_sim *sim, const f110_map *map, const f110_be
                          const double *actions_host, double *actions_dev_scratch, const f110_host_obs *stage,
                          const f110_host_obs *out, void *compute_stream, void *copy_stream, void *ev_tick_done,
                          void *ev_copy_done) {
+    return f110_step_host_async_ex(sim, map, nullptr, beams, actions_host, actions_dev_scratch, stage, out, compute_stream,
+                                   copy_stream, ev_tick_done, ev_copy_done);
+}
+int f110_step_host_async_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables,
+                            const f110_beams *beams, const double *actions_host, double *actions_dev_scratch,
+                            const f110_host_obs *stage, const f110_host_obs *out, void *compute_stream, void *copy_stream,
+                            void *ev_tick_done, void *ev_copy_done) {
     int rc;
     if ((rc = check_sim(sim))) return rc;
     if (!actions_host || !actions_dev_scratch || !stage || !out || !ev_tick_done || !ev_copy_done) return F110_ERR_INVALID;
@@ -1886,7 +1949,7 @@ int f110_step_host_async(const f110_sim *sim, const f110_map *map, const f110_be
     TailOpts t;
     t.fused = true; t.env_level = env_level ? 1 : 0;
     t.ar.start_poses = nullptr; t.ar.num_start = 0; t.ar.pose_gap = 0; t.ar.seed = 0; t.ar.tick_host = 0;
-    if ((rc = step_impl(sim, map, beams, actions_dev_scratch, cs, nullptr, &t))) return rc;
+    if ((rc = step_impl(sim, map, tables, beams, actions_dev_scratch, cs, nullptr, &t))) return rc;
     // the staging buffers may still be draining to the host from their previous use
     CUDA_TRY(cudaStreamWaitEvent(cs, e_copy, 0));
     struct Part { void *dst_dev, *dst_host; const void *src; size_t bytes; };
@@ -1912,6 +1975,23 @@ int f110_step_host_async(const f110_sim *sim, const f110_map *map, const f110_be
     if (packed)
         CUDA_TRY(cudaMemcpyAsync(out->scans_u24, stage->scans_u24, NA * beams->num_beams * 3, cudaMemcpyDeviceToHost, ps));
     CUDA_TRY(cudaEventRecord(e_copy, ps));
+    return F110_OK;
+}
+
+int64_t f110_map_brick_elems(const f110_map *map) {
+    if (!map || !map->dt_cells_pad || !map->fast_path || map->num_layers > 1 || map->layer_geom || map->height < 1 ||
+        map->width < 1)
+        return 0;
+    return (int64_t)brick_elems(map);
+}
+
+int f110_map_brick(const f110_map *map, double *out, void *stream) {
+    const int64_t n = f110_map_brick_elems(map);
+    if (n <= 0 || !out) return F110_ERR_INVALID;
+    k_map_brick<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(map->dt_cells_pad, (unsigned)map->height,
+                                                                                 (unsigned)map->width, (unsigned)brick_cols(map),
+                                                                                 out, (unsigned)n);
+    LAUNCH_CHECK("k_map_brick");
     return F110_OK;
 }
 

@@ -51,10 +51,31 @@ struct LeanK {
     int B;
     // literal fallback for absurd coordinates
     const double *__restrict__ dt;
-    double orig_x, orig_y, dt_oob_unused, eps_m, max_range;
+    double orig_x, orig_y;
+    unsigned brick_cols1, unused;           // k_march_lean_brick: bricks per row of the brick table, minus one
+    double eps_m, max_range;
     unsigned long long layer_stride;        // elements between layers of dt (metres table)
     unsigned long long layer_stride_lean;   // elements between layers of `table`
 };
+
+// Element (r, c) of the padded (H+1) x (W+1) cell-unit table in the brick table (f110_march_tables.dt_cells_brick): bricks of
+// 4 x 4 cells (128 bytes of fp64, one cache line), row-major over a grid of bw = brick_cols1 + 1 bricks per row, and row-major
+// inside a brick: ((r / 4) * bw + c / 4) * 16 + (r % 4) * 4 + c % 4, rearranged to two AND and two multiply-adds
+__device__ __forceinline__ unsigned brick_index(unsigned r, unsigned c, unsigned brick_cols1) {
+    return ((r & ~3u) * brick_cols1 + r) * 4u + (c & ~3u) * 3u + c;
+}
+
+// f110_map_brick: the brick table from the padded row-major table (height + 1 rows of width + 1), thread per element.  Element e
+// holds cell (r, c) = ((e / 16) / bw * 4 + e % 16 / 4, (e / 16) % bw * 4 + e % 4); cells beyond the padded table (the rows and
+// columns that round it up to whole bricks) hold its last element, dt[-1,-1] / resolution, like the padding itself
+__global__ void k_map_brick(const double *__restrict__ pad, unsigned height, unsigned width, unsigned bw, double *__restrict__ out,
+                            unsigned n) {
+    const unsigned e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const unsigned b = e >> 4;
+    const unsigned r = (b / bw) * 4u + ((e >> 2) & 3u), c = (b % bw) * 4u + (e & 3u);
+    out[e] = (r <= height && c <= width) ? pad[r * (width + 1u) + c] : pad[height * (width + 1u) + width];
+}
 
 // per-agent record, 4 x double2:
 //   [0] (X, Y)      scan position: cell units (CELLS) or metres
@@ -207,8 +228,10 @@ __device__ __noinline__ unsigned dyn_queue_position_zoned(unsigned k, bool elect
 // IPT: queue entries per ticket (1, 2 or 4; 0 = by the class of the run, mq.ipt_shifts, dynamic queue only).  With 2, a warp that
 // pops the block's counter marches two consecutive entries of its run before it pops again: the pop, the queue arithmetic and
 // the dynamic-queue call are paid once per 64 beams.
-template <int TABLE, bool NOISE, bool COUNT, bool CELLS, bool LAYERED, int PT, int MINB, bool DYN = false, int CL = 1, int IPT = 1, int RING = 0>
-__global__ void __launch_bounds__(PT, MINB) k_march_lean(const LeanK p, const MarchQueue mq) {
+// BRICK (k_march_lean_brick): `table` is the same padded cell-unit table stored in 4 x 4-cell bricks (brick_index)
+template <int TABLE, bool NOISE, bool COUNT, bool CELLS, bool LAYERED, int PT, int MINB, bool DYN, int CL, int IPT, int RING, bool BRICK>
+__device__ __forceinline__ void march_lean_body(const LeanK &p, const MarchQueue &mq) {
+    static_assert(!BRICK || (TABLE == 0 && CELLS && !LAYERED), "the brick table is a single fp64 cell-unit map");
     __shared__ unsigned s_next;
     __shared__ unsigned s_run[DYN ? F110_DYN_RING : 1u], s_seq[DYN ? F110_DYN_RING : 1u];
     if (DYN && threadIdx.x < F110_DYN_RING) s_seq[threadIdx.x] = 0xFFFFFFFFu;
@@ -321,6 +344,7 @@ __global__ void __launch_bounds__(PT, MINB) k_march_lean(const LeanK p, const Ma
                             const unsigned r = (unsigned)__double2loint(__dadd_rd(Y - p.oy, MAGIC));
                             // off-map -> the padding row / column, which holds dt[-1,-1]
                             if (TABLE == 1) D = s_lut[__ldg(p.codes + min(r, p.height) * p.codes_pitch + min(c, p.width))];
+                            else if (BRICK) D = __ldg(table + brick_index(min(r, p.height), min(c, p.width), p.brick_cols1));
                             else D = __ldg(table + min(r, p.height) * (p.width + 1u) + min(c, p.width));
                             T = T + D;
                             n++;
@@ -383,6 +407,17 @@ __global__ void __launch_bounds__(PT, MINB) k_march_lean(const LeanK p, const Ma
     }
     // the rank-0 CTA's shared memory must outlive the last pop of every CTA of the cluster
     if (CL > 1) asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+
+template <int TABLE, bool NOISE, bool COUNT, bool CELLS, bool LAYERED, int PT, int MINB, bool DYN = false, int CL = 1, int IPT = 1, int RING = 0>
+__global__ void __launch_bounds__(PT, MINB) k_march_lean(const LeanK p, const MarchQueue mq) {
+    march_lean_body<TABLE, NOISE, COUNT, CELLS, LAYERED, PT, MINB, DYN, CL, IPT, RING, false>(p, mq);
+}
+
+// k_march_lean on the bricked cell-unit table (f110_march_tables.dt_cells_brick): one fp64 map in cell units, not layered
+template <bool NOISE, bool COUNT, int PT, int MINB, bool DYN, int IPT, int RING>
+__global__ void __launch_bounds__(PT, MINB) k_march_lean_brick(const LeanK p, const MarchQueue mq) {
+    march_lean_body<0, NOISE, COUNT, true, false, PT, MINB, DYN, 1, IPT, RING, true>(p, mq);
 }
 
 }  // namespace f110

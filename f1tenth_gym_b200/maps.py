@@ -80,6 +80,32 @@ def code_table(values, ncodes=255):
     return np.ascontiguousarray(codes), lut
 
 
+def pad_table(cells):
+    """[H][W] cell-unit table -> [H+1][W+1] with the extra row and column holding cells[-1,-1], the value an off-map lookup
+    reads (host model of DeviceMap._pad, f110_map.dt_cells_pad)."""
+    H, W = cells.shape
+    out = np.full((H + 1, W + 1), cells[-1, -1], dtype=cells.dtype)
+    out[:H, :W] = cells
+    return out
+
+
+def brick_table(pad):
+    """Host model of f110_map_brick (f110_march_tables.dt_cells_brick): the padded table [H+1][W+1] stored in 4 x 4-cell
+    bricks, flat [ceil((H+1)/4) * ceil((W+1)/4) * 16]; the cells that round it up to whole bricks hold pad[-1,-1]."""
+    Hp, Wp = pad.shape
+    R, C = -(-Hp // 4), -(-Wp // 4)
+    full = np.full((4 * R, 4 * C), pad[-1, -1], dtype=pad.dtype)
+    full[:Hp, :Wp] = pad
+    return np.ascontiguousarray(full.reshape(R, 4, C, 4).transpose(0, 2, 1, 3)).reshape(-1)
+
+
+def brick_index(r, c, width):
+    """Index of cell (r, c) of the padded table (r <= height, c <= width) in brick_table, in the kernel's form
+    (csrc/march_lean.cuh brick_index): ((r / 4) * bw + c / 4) * 16 + (r % 4) * 4 + c % 4 with bw = ceil((width + 1) / 4)."""
+    bw1 = (width + 4) // 4 - 1
+    return ((r & ~3) * bw1 + r) * 4 + (c & ~3) * 3 + c
+
+
 def load_bitmap(map_path, map_ext):
     """Image + yaml part of ScanSimulator2D.set_map (laser_models.py:397-422): returns (bitmap {0,255} fp64 with
     row 0 = image bottom, resolution, origin)."""

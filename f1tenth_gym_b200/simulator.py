@@ -78,6 +78,13 @@ class DeviceMap(object):
                              nat.ptr(self.sincos), nat.ptr(self.dt_cells_pad), nat.ptr(self.dt_codes_pad),
                              0 if self.dt_codes_pad is None else self.dt_codes_pad.shape[1],
                              nat.ptr(self.sincos2), dt_min_positive, 1)
+        # the padded cell-unit table again in 4 x 4-cell bricks (f110_map_brick): what the ray march of the tick reads
+        self.dt_cells_brick = None
+        n = nat.lib().f110_map_brick_elems(C.byref(self.c)) if self.dt_cells_pad is not None and self.dt_cells_pad.is_cuda else 0
+        if n > 0:
+            self.dt_cells_brick = torch.empty((n,), dtype=torch.float64, device=device)
+            nat.check(nat.lib().f110_map_brick(C.byref(self.c), nat.ptr(self.dt_cells_brick), _stream_ptr(self.dt_cells_pad.device)))
+        self.march_tables = nat.F110MarchTables(nat.ptr(self.dt_cells_brick))
 
     @staticmethod
     def _pad(t, pitch_multiple=1):
@@ -120,6 +127,8 @@ class DeviceMap(object):
         out.dt_cells = torch.stack([m.dt_cells for m in maps]).contiguous() if m0.dt_cells is not None else None
         out.dt_cells_pad = torch.stack([m.dt_cells_pad for m in maps]).contiguous() if m0.dt_cells_pad is not None else None
         out.dt_codes = out.dt_lut = out.dt_codes_pad = None
+        out.dt_cells_brick = None           # the brick table is built for a single map only
+        out.march_tables = nat.F110MarchTables()
         c = nat.F110Map.from_buffer_copy(m0.c)
         c.dt = nat.ptr(out.dt)
         c.dt_cells = nat.ptr(out.dt_cells)
@@ -171,6 +180,8 @@ class DeviceMap(object):
         out.dt_cells = canvas([m.dt_cells for m in maps], 0) if cells else None
         out.dt_cells_pad = canvas([m.dt_cells for m in maps], 1) if cells else None
         out.dt_codes = out.dt_lut = out.dt_codes_pad = None
+        out.dt_cells_brick = None
+        out.march_tables = nat.F110MarchTables()
         out.layer_geom_host = np.array([[h.orig_x, h.orig_y, h.width * h.resolution, h.height * h.resolution, h.width,
                                          h.height] for h in hs], dtype=np.float64)
         out.layer_geom = torch.from_numpy(out.layer_geom_host).to(maps[0].device)
@@ -356,6 +367,7 @@ class Simulator(object):
         self.map = None
         self.env_layer = None
         self._map_struct = empty_map_struct()
+        self._march_tables = nat.F110MarchTables()
         self._actions_dev = torch.zeros((NA, 2), **f64)
         self.c = nat.F110Sim(
             N, A, integ, ego_idx, 0, time_step, lidar_dist, 0.005, float(params['length']), float(params['width']),
@@ -384,6 +396,7 @@ class Simulator(object):
         """env_map_ids (N,) ints: which layer of a DeviceMap.stack() each env uses (multi-map batches)."""
         self.map = device_map
         self._map_struct = device_map.c
+        self._march_tables = getattr(device_map, 'march_tables', None) or nat.F110MarchTables()
         self._graph = None
         self.set_centerlines(None)      # the centerlines belong to the old map
         layers = getattr(device_map.c, 'num_layers', 1)
@@ -501,8 +514,8 @@ class Simulator(object):
     def step(self, control_inputs):
         """Simulator.step (base_classes.py:553-612). control_inputs (N,A,2) = (steer, speed)."""
         a = self._actions_tensor(control_inputs)
-        nat.check(nat.lib().f110_step(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c),
-                                      nat.ptr(a), _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_step_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                         C.byref(self.beams.c), nat.ptr(a), _stream_ptr(self.device)))
         return self.observations()
 
     def env_post_step(self):
@@ -542,9 +555,9 @@ class Simulator(object):
         results as step(); env_post_step(); autoreset()."""
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
-        nat.check(nat.lib().f110_tick(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c), nat.ptr(a),
-                                      1 if env_level else 0, nat.ptr(table), n, pose_gap, int(seed),
-                                      _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_tick_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                         C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
+                                         int(seed), _stream_ptr(self.device)))
         return self.observations()
 
     def observations(self):
@@ -723,9 +736,9 @@ class Simulator(object):
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
 
         def tick():
-            nat.check(L.f110_tick(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c), nat.ptr(actions),
-                                  1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(autoreset_seed),
-                                  _stream_ptr(self.device)))
+            nat.check(L.f110_tick_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                     C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
+                                     pose_gap, int(autoreset_seed), _stream_ptr(self.device)))
             if progress:
                 self._launch_progress(L)
         side = torch.cuda.Stream(self.device)
@@ -817,8 +830,8 @@ class Simulator(object):
     def step_host_async(self, io):
         """Enqueue one tick whose observation lands in io's pinned host buffers (C ABI f110_step_host_async);
         returns immediately.  Call wait_host(io) before reading them or before reusing io."""
-        nat.check(nat.lib().f110_step_host_async(
-            C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c), nat.ptr(io['actions']),
+        nat.check(nat.lib().f110_step_host_async_ex(
+            C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables), C.byref(self.beams.c), nat.ptr(io['actions']),
             nat.ptr(io['_actions_dev']), C.byref(io['_stage_struct']), C.byref(io['_struct']),
             _stream_ptr(self.device), C.c_void_p(io['_copy_stream'].cuda_stream),
             C.c_void_p(io['_ev_tick'].cuda_event), C.c_void_p(io['_ev_copy'].cuda_event)))
@@ -832,8 +845,8 @@ class Simulator(object):
         """One tick with CUDA events around each kernel -> (dynamics_ms, raymarch_ms, finalize_ms)."""
         a = self._actions_tensor(control_inputs)
         ms = (C.c_float * 3)()
-        nat.check(nat.lib().f110_step_profile(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c),
-                                              nat.ptr(a), ms, _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_step_profile_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                                 C.byref(self.beams.c), nat.ptr(a), ms, _stream_ptr(self.device)))
         return float(ms[0]), float(ms[1]), float(ms[2])
 
     def lookups(self):

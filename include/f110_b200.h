@@ -166,19 +166,43 @@ int f110_abi_version(void);
 const char *f110_status_string(int status);
 const char *f110_last_cuda_error(void);
 
+/* Optional copies of a map's tables in other layouts, read only by the ray march of the tick.  Held apart from f110_map so
+ * that its layout stays that of ABI v6; every pointer may be NULL (the tick then reads the f110_map tables alone). */
+typedef struct {
+    const double *dt_cells_brick;   /* f110_map.dt_cells_pad stored in 4x4-cell bricks (one 128-byte line each), built by
+                                       f110_map_brick: element (r, c) at ((r/4)*BW + c/4)*16 + (r%4)*4 + c%4 with
+                                       BW = ceil((width+1)/4); the rows are padded to a multiple of 4 and every cell beyond the
+                                       padded table holds dt[-1,-1]/resolution.  Read by the ray march of a single fast-path map
+                                       (num_layers <= 1, no layer_geom) at up to 1080 beams in place of dt_cells_pad; ignored
+                                       on any other map and at more beams */
+} f110_march_tables;
+
+/* Size in elements of the brick table of `map`: ceil((height+1)/4)*4 * ceil((width+1)/4)*4, or 0 when the map has no brick
+ * table (no dt_cells_pad, not a fast-path map, or a stack of layers) or it would hold 2^32 elements or more. */
+int64_t f110_map_brick_elems(const f110_map *map);
+/* Write the brick table of `map` (f110_march_tables.dt_cells_brick) into `out` (device, f110_map_brick_elems(map) fp64)
+ * from map->dt_cells_pad on `stream`: a copy, bit for bit.  F110_ERR_INVALID when f110_map_brick_elems(map) is 0. */
+int f110_map_brick(const f110_map *map, double *out, void *stream);
+
 /* ---- the per-tick hot path -------------------------------------------------------------------- */
+/* Each of f110_step, f110_step_profile, f110_tick and f110_step_host_async has an *_ex sibling that also takes the optional
+ * tables (`tables` may be NULL: same as the plain entry point).  Results never depend on the tables; only speed does. */
 
 /* Simulator.step (base_classes.py:553-612): pid + RK4/Euler dynamics -> 1080-beam ray-march (+fused
  * iTTC) -> GJK, wall-hit state zeroing, opponent ray-cast.  actions: device [N*A][2] = (steer, speed).
  * Launches 3 kernels on `stream`; no host synchronisation. */
 int f110_step(const f110_sim *sim, const f110_map *map, const f110_beams *beams,
               const double *actions, void *stream);
+int f110_step_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                 const double *actions, void *stream);
 
 /* f110_step with CUDA events recorded on `stream` around each of its three kernels; synchronises and
  * returns their durations in milliseconds: kernel_ms[0..2] = dynamics, ray-march, finalize (host array).
  * Measurement aid for bench.py's roofline figure; not for the hot loop. */
 int f110_step_profile(const f110_sim *sim, const f110_map *map, const f110_beams *beams,
                       const double *actions, float *kernel_ms, void *stream);
+int f110_step_profile_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables,
+                         const f110_beams *beams, const double *actions, float *kernel_ms, void *stream);
 
 /* Simulator.reset / RaceCar.reset (base_classes.py:183-204, 614-630) for the envs whose env_mask
  * byte is non-zero (env_mask == NULL: all).  poses: device [N*A][3].  No tick is executed. */
@@ -209,6 +233,9 @@ int f110_autoreset(const f110_sim *sim, const double *start_poses, int32_t num_s
 int f110_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
               int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
               void *stream);
+int f110_tick_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                 const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                 uint64_t seed, void *stream);
 
 /* Same tick through HOST buffers: copies actions H2D, runs f110_step (+ f110_env_post_step when the
  * lap arrays are bound), copies the observation D2H and synchronises the stream.
@@ -239,6 +266,10 @@ int f110_step_host_async(const f110_sim *sim, const f110_map *map, const f110_be
                          const double *actions_host, double *actions_dev_scratch, const f110_host_obs *stage,
                          const f110_host_obs *out, void *compute_stream, void *copy_stream, void *ev_tick_done,
                          void *ev_copy_done);
+int f110_step_host_async_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables,
+                            const f110_beams *beams, const double *actions_host, double *actions_dev_scratch,
+                            const f110_host_obs *stage, const f110_host_obs *out, void *compute_stream, void *copy_stream,
+                            void *ev_tick_done, void *ev_copy_done);
 
 /* scans [count] fp32 (device) -> out [count][3] bytes (device): q = round(range * 2^19) clamped to [0, 2^24-1], little endian.
  * No reference counterpart (the reference hands numpy arrays to a policy in the same process); batch extension for host-side

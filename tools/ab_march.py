@@ -11,7 +11,9 @@ statically and the rest claimed dynamically (--dyn static_pct:ahead); 66 / 60 / 
 threads per SM; 42 dynamic with 2 x 1024; 62-65 thread-block clusters sharing
 one ticket counter through DSMEM; 40 / 41 dynamic queue tail; 30 / 31 TMA tile; 21 lean at 48 warps/SM (40 registers);
 20 / 22 lean, u8 rank-coded table + shared-memory LUT (64 / 48 warps); 1 round-1 persistent kernel; 6 round-1 coded;
-7 no queue (block per 64-beam tile); 30+ see csrc/f110_b200.cu.
+7 no queue (block per 64-beam tile); 90 the padded row-major table instead of the 4 x 4-cell brick table (f110_march_tables);
+30+ see csrc/f110_b200.cu.
+The first and last lines name the card with its power limit and SM clock (nvidia-smi, read only).
 """
 import argparse
 import ctypes as C
@@ -23,6 +25,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import re
+import subprocess
 
 import numpy as np   # noqa: E402
 import torch         # noqa: E402
@@ -92,6 +95,16 @@ def run(workload, variant, ticks, dev, chunk=3, dyn=(50, 4), pdl=0, tail=8, tail
             'hash': h.hexdigest()[:16]}
 
 
+def card():
+    q = 'name,power.limit,clocks.sm,clocks.max.sm,temperature.gpu'
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=' + q, '--format=csv,noheader', '-i', '0'], capture_output=True,
+                             text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        out = 'nvidia-smi failed: %s' % e
+    return {'card': torch.cuda.get_device_name(0), 'nvidia_smi': dict(zip(q.split(','), [x.strip() for x in out.split(',')]))}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--workloads', default='cfg2,cfg2x2,cfg3')
@@ -106,6 +119,7 @@ def main():
     ap.add_argument('--repeat', type=int, default=2)
     args = ap.parse_args()
     dev = torch.device('cuda:0')
+    print(json.dumps(card()), flush=True)
     rows = []
     for wl in args.workloads.split(','):
         for rep in range(args.repeat):
@@ -123,6 +137,7 @@ def main():
                                         print(json.dumps(r), flush=True)
         hs = {r['hash'] for r in rows if r['workload'] == wl}
         print(json.dumps({'workload': wl, 'identical_results_across_variants': len(hs) == 1}), flush=True)
+    print(json.dumps(card()), flush=True)
 
 
 if __name__ == '__main__':
