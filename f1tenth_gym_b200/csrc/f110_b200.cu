@@ -394,6 +394,9 @@ __global__ void __launch_bounds__(256) k_raymarch(MapView m, BeamView bv, MarchA
 }
 
 // ------------------------------------------------------------------------------------ finalize
+// an angle difference reduced to [-pi, pi] (up to rounding), for any finite input
+__device__ __forceinline__ double wrap_2pi_diff(double d) { return d - (2 * M_PI) * rint(d * (1.0 / (2 * M_PI))); }
+
 // One warp finalises one agent (base_classes.py:536-550 check_collision, :579-589 update_scan loop).
 __device__ __forceinline__ void finalize_agent(const f110_sim &s, const BeamView &bv, int a, int lane,
                                                double max_scan_range) {
@@ -502,7 +505,10 @@ __device__ __forceinline__ void finalize_agent(const f110_sim &s, const BeamView
                 // the direction to the opponent, or of the opposite direction, can pass the test above.  Those are the
                 // beams around the centres (phi - yaw) + m pi; visit just these index intervals, with two beams of slack
                 // on both sides -- the exact per-beam test still decides.
-                const double base = phi - yaw, half = bv.fov / 2., inv_inc = 1.0 / bv.angle_increment;
+                // (phi - yaw reduced modulo 2 pi: the state's yaw is wrapped once per step only, so an integration that blows
+                // up -- e.g. the single-track model at a 0.05 s time step -- leaves it anywhere, and the clamped m range below
+                // would then miss the centres)
+                const double base = wrap_2pi_diff(phi - yaw), half = bv.fov / 2., inv_inc = 1.0 / bv.angle_increment;
                 // centres base + m pi that can reach the beam range [-half, half] (+- cone and slack): usually 1-3 of them
                 const int m0 = max(-3, (int)floor((-half - cone - 0.02 - base) * (1.0 / M_PI))),
                           m1 = min(5, (int)ceil((half + cone + 0.02 - base) * (1.0 / M_PI)));
@@ -839,7 +845,7 @@ __global__ void __launch_bounds__(F110_TAIL2_THREADS, 3) k_tail2(f110_sim s, Bea
                 }
             };
             if (cone < 3.5 && hi - lo >= 96) {
-                const double base = phi - yaw, half = bv.fov / 2., inv_inc = 1.0 / bv.angle_increment;
+                const double base = wrap_2pi_diff(phi - yaw), half = bv.fov / 2., inv_inc = 1.0 / bv.angle_increment;   // (see finalize_agent)
                 const int m0 = max(-3, (int)floor((-half - cone - 0.02 - base) * (1.0 / M_PI))),
                           m1 = min(5, (int)ceil((half + cone + 0.02 - base) * (1.0 / M_PI)));
                 for (int m = m0; m <= m1; m++) {

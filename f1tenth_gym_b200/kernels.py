@@ -19,7 +19,7 @@ import torch
 
 from . import _native as nat
 from . import maps as hostmaps
-from .simulator import DeviceBeams, DeviceMap, _stream_ptr
+from .simulator import DeviceBeams, DeviceMap, _stream_ptr, check_theta_dis
 
 
 def _dev(t, dtype=torch.float64, device=None):
@@ -142,7 +142,9 @@ class ScanSimulator2D(object):
         return True
 
     def set_device_map(self, device_map):
-        """A DeviceMap built elsewhere (device EDT, generated track) instead of a yaml + image on disk."""
+        """A DeviceMap built elsewhere (device EDT, generated track) instead of a yaml + image on disk.  ValueError for a map
+        built with another theta_dis than this scan simulator's (its beam tables would step through the wrong LUT)."""
+        check_theta_dis(device_map, self.theta_dis, 'ScanSimulator2D')
         self.map = device_map
         self.map_height, self.map_width = device_map.host.height, device_map.host.width
         self.map_resolution = device_map.host.resolution

@@ -27,6 +27,7 @@ from . import maps as hostmaps
 RENDER_MAX_AGENTS = 64     # csrc/render.cuh F110_RENDER_MAX_AGENTS: car quads a block of k_render_views caches
 RENDER_MAX_SIZE = 8192     # largest view height / width of f110_render_views
 TRACK_MAX_WINDOW = 1024    # csrc/progress.cuh F110_TRACK_MAX_WINDOW: largest back + fwd + 1 of the progress tracker
+PACKED_RANGE_LIMIT = 32.0  # f110_pack_scans_u24: 24 bits of 2^-19 m clamp every range at 32 m - 2^-19
 
 
 class Integrator(Enum):     # base_classes.py:40-42
@@ -107,9 +108,15 @@ class DeviceMap(object):
         the flag changes nothing.
         Maps whose origin has a yaw raise ValueError unless rotated_origins=True: then the maps are stacked on a metre canvas
         with each layer's own resolution and rotation (see _stack_canvas), marched by k_march_lean_rot; different
-        resolutions still also need mixed_resolution=True.  Without a rotated map the flag changes nothing."""
+        resolutions still also need mixed_resolution=True.  Without a rotated map the flag changes nothing.
+        Every layer must share theta_dis, eps and max_range (ValueError otherwise): the stack keeps one LUT and one set of
+        march constants, the first map's."""
         m0 = maps[0]
         h0 = m0.host
+        for m in maps[1:]:
+            for k in ('theta_dis', 'eps', 'max_range'):
+                if getattr(m.c, k) != getattr(m0.c, k):
+                    raise ValueError('stacked maps must share %s: %r and %r' % (k, getattr(m0.c, k), getattr(m.c, k)))
         if len(maps) > 1 and any(m.host.orig_c != 1.0 or m.host.orig_s != 0.0 for m in maps):
             if not rotated_origins:
                 raise ValueError('stacking maps with a rotated origin needs rotated_origins=True')
@@ -289,6 +296,15 @@ class CenterlineTables(object):
         self.c = nat.F110Track(self.num_tables, min(self.num_segments), nat.ptr(self.table_start), nat.ptr(self.segments))
 
 
+def check_theta_dis(device_map, theta_dis, who):
+    """ValueError unless device_map's sin / cos LUT has theta_dis entries: beam tables built for one theta_dis step through
+    another's LUT with the wrong increment, so every beam after the first would point the wrong way."""
+    got = int(device_map.c.theta_dis)
+    if got != int(theta_dis):
+        raise ValueError('the map was built with theta_dis=%d but this %s has theta_dis=%d; build both with the same value'
+                         % (got, who, int(theta_dis)))
+
+
 def empty_map_struct():
     """A map struct with no DT bound: stepping with it raises ValueError like the reference
     (laser_models.py:445-446 'Map is not set for scan simulator.')."""
@@ -303,7 +319,9 @@ class Simulator(object):
 
     def __init__(self, params, num_agents, seed, time_step=0.01, ego_idx=0, integrator=Integrator.RK4,
                  lidar_dist=0.0, num_envs=1, num_beams=1080, fov=4.7, device=None, noise_std=0.0,
-                 count_lookups=False, march_queue=True, march_item_beams=32):
+                 count_lookups=False, march_queue=True, march_item_beams=32, theta_dis=2000):
+        """theta_dis: entries of the map's sin / cos LUT (ScanSimulator2D's theta_dis) that the beam tables step through;
+        set_device_map refuses a map built for another value."""
         nat.lib()   # fail loudly right away if the CUDA library is missing
         if device is None:
             device = torch.device('cuda', torch.cuda.current_device())
@@ -317,6 +335,7 @@ class Simulator(object):
         self.integrator = integrator
         self.lidar_dist = lidar_dist
         self.num_beams, self.fov = num_beams, fov
+        self.theta_dis = int(theta_dis)
         if isinstance(integrator, Integrator):
             integ = integrator.value
         elif integrator in (1, 2):
@@ -363,7 +382,7 @@ class Simulator(object):
         self.march_order = torch.zeros((3, items), **i32) if self.march_ipa else None
         self.march_count = torch.zeros((4,), **i32) if self.march_ipa else None
         self.march_rec = torch.zeros((NA, 8), **f64) if self.march_ipa else None
-        self.beams = DeviceBeams(num_beams, fov, params, dev)
+        self.beams = DeviceBeams(num_beams, fov, params, dev, self.theta_dis)
         self.map = None
         self.env_layer = None
         self._map_struct = empty_map_struct()
@@ -390,10 +409,12 @@ class Simulator(object):
     def set_map(self, map_path, map_ext, edt='scipy'):
         """base_classes.py:499-511 / laser_models.py:383-427 (load-time: PIL + yaml + EDT; edt='device' runs the
         exact distance transform on the GPU instead of scipy on the host)."""
-        self.set_device_map(DeviceMap.from_yaml(map_path, map_ext, self.device, edt=edt))
+        self.set_device_map(DeviceMap.from_yaml(map_path, map_ext, self.device, edt=edt, theta_dis=self.theta_dis))
 
     def set_device_map(self, device_map, env_map_ids=None):
-        """env_map_ids (N,) ints: which layer of a DeviceMap.stack() each env uses (multi-map batches)."""
+        """env_map_ids (N,) ints: which layer of a DeviceMap.stack() each env uses (multi-map batches).  ValueError for a map
+        whose theta_dis differs from the simulator's: the beams would step through its LUT with the wrong increment."""
+        check_theta_dis(device_map, self.theta_dis, 'Simulator')
         self.map = device_map
         self._map_struct = device_map.c
         self._march_tables = getattr(device_map, 'march_tables', None) or nat.F110MarchTables()
@@ -796,14 +817,17 @@ class Simulator(object):
 
     def make_host_pipeline(self, depth=2, with_scans=True, packed_scans=False):
         """`depth` independent sets of (pinned host obs, device staging, events, actions scratch) for
-        step_host_async(); one shared copy stream."""
+        step_host_async(); one shared copy stream.  packed_scans=True: ValueError for a map whose max_range plus 8 sigma of
+        the scan noise reaches 32 m, where the 24-bit block clamps (step_host_async checks again once the map or the noise
+        changed)."""
         N, A, B = self.num_envs, self.num_agents, self.num_beams
         NA = N * A
         dev = self.device
-        copy_stream = torch.cuda.Stream(dev)
         sets = []
         if packed_scans:
             with_scans = False
+            self._check_packed_range()
+        copy_stream = torch.cuda.Stream(dev)
         for _ in range(depth):
             io = self.make_host_io(with_scans, packed_scans)
             st = {'scans': torch.zeros((NA, B), dtype=torch.float32, device=dev) if with_scans else None,
@@ -823,13 +847,30 @@ class Simulator(object):
             io['_ev_tick'].record()
             io['_ev_copy'].record()
             io['_copy_stream'] = copy_stream
+            io['_packed_checked'] = (self._map_struct, self.c.noise_std) if packed_scans else None
             sets.append(io)
         torch.cuda.synchronize(dev)
         return sets
 
+    def _check_packed_range(self):
+        """ValueError unless every range of the current map (max_range plus 8 sigma of the scan noise) stays below the 32 m
+        where the 24-bit scan block clamps."""
+        if self.map is None:
+            return
+        top = float(self._map_struct.max_range) + 8.0 * max(float(self.c.noise_std), 0.0)
+        if not top < PACKED_RANGE_LIMIT:
+            raise ValueError('packed_scans holds ranges below %g m only, but this map reaches max_range + 8 * noise_std = %g m'
+                             % (PACKED_RANGE_LIMIT, top))
+
     def step_host_async(self, io):
         """Enqueue one tick whose observation lands in io's pinned host buffers (C ABI f110_step_host_async);
-        returns immediately.  Call wait_host(io) before reading them or before reusing io."""
+        returns immediately.  Call wait_host(io) before reading them or before reusing io.  With a packed io, ValueError
+        (before anything is enqueued) when the map or the noise changed since the last check and now reaches 32 m."""
+        if io['scans_u24'] is not None:
+            checked = io.get('_packed_checked')
+            if checked is None or checked[0] is not self._map_struct or checked[1] != self.c.noise_std:
+                self._check_packed_range()
+                io['_packed_checked'] = (self._map_struct, self.c.noise_std)
         nat.check(nat.lib().f110_step_host_async_ex(
             C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables), C.byref(self.beams.c), nat.ptr(io['actions']),
             nat.ptr(io['_actions_dev']), C.byref(io['_stage_struct']), C.byref(io['_struct']),

@@ -273,7 +273,9 @@ int f110_step_host_async_ex(const f110_sim *sim, const f110_map *map, const f110
 
 /* scans [count] fp32 (device) -> out [count][3] bytes (device): q = round(range * 2^19) clamped to [0, 2^24-1], little endian.
  * No reference counterpart (the reference hands numpy arrays to a policy in the same process); batch extension for host-side
- * consumers behind PCIe.  Decode: (b0 | b1 << 8 | b2 << 16) * 2^-19. */
+ * consumers behind PCIe.  Decode: (b0 | b1 << 8 | b2 << 16) * 2^-19.
+ * The clamp: every range at or above 32 - 2^-19 m decodes to 32 - 2^-19 m, so the block only holds scans of a map whose
+ * max_range plus the noise head-room stays below 32 m (the Python pipeline refuses any other map). */
 int f110_pack_scans_u24(const float *scans, int64_t count, uint8_t *out, void *stream);
 
 /* ---- standalone kernels (unit-parity surface; device pointers) ------------------------------- */

@@ -66,6 +66,8 @@ def lib():
         L.orc_sim_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double,
                                      C.c_double, C.POINTER(_Map), _dp, _dp, _dp, _dp]
         L.orc_sim_destroy.argtypes = [C.c_void_p]
+        L.orc_sim_set_ego.argtypes = [C.c_void_p, C.c_int]
+        L.orc_sim_set_ego.restype = C.c_int
         for name in ('state', 'scans', 'collisions', 'collision_idx', 'lap_times', 'lap_counts',
                      'toggle_list', 'params', 'steer_buf'):
             f = getattr(L, 'orc_sim_' + name)
@@ -257,16 +259,22 @@ class OracleSim(object):
     """One environment: base_classes.Simulator semantics (+ F110Env lap logic)."""
 
     def __init__(self, omap, params=None, num_agents=2, num_beams=1080, fov=4.7, timestep=0.01,
-                 integrator=1, lidar_dist=0.0):
+                 integrator=1, lidar_dist=0.0, ego_idx=0):
+        """ego_idx: F110Env's ego (f110_env.py:145): its collision sets `done`, its start yaw the lap frame."""
         params = dict(DEFAULT_PARAMS) if params is None else params
+        if not 0 <= ego_idx < num_agents:
+            raise ValueError('ego_idx %r outside [0, %d)' % (ego_idx, num_agents))
         self.omap = omap
         self.num_agents, self.num_beams = num_agents, num_beams
+        self.ego_idx = ego_idx
         self._tabs = beam_tables(num_beams, fov, params)
         pv = np.tile(params_vector(params), (num_agents, 1))
         self._h = lib().orc_sim_create(num_agents, num_beams, integrator, timestep, fov,
                                        theta_index_increment(num_beams, fov, omap.theta_dis),
                                        lidar_dist, C.byref(omap.c), _p(self._tabs[0]),
                                        _p(self._tabs[1]), _p(self._tabs[2]), _p(pv))
+        if lib().orc_sim_set_ego(self._h, ego_idx) != 0:
+            raise ValueError('orc_sim_set_ego refused ego_idx %r' % ego_idx)
         A, B = num_agents, num_beams
         L = lib()
         h = self._h

@@ -443,6 +443,14 @@ orc_sim_t *orc_sim_create(int num_agents, int num_beams, int integrator, double 
     return s;
 }
 
+/* F110Env(ego_idx=...) (f110_env.py:145): the agent whose collision ends the episode and whose start pose sets the lap
+ * frame.  orc_sim_create starts with agent 0.  Returns 0, or -1 (nothing changed) for an index outside [0, num_agents). */
+int orc_sim_set_ego(orc_sim_t *s, int ego_idx) {
+    if (ego_idx < 0 || ego_idx >= s->num_agents) return -1;
+    s->ego_idx = ego_idx;
+    return 0;
+}
+
 void orc_sim_destroy(orc_sim_t *s) {
     if (!s) return;
     free(s->params); free(s->state); free(s->steer_buf); free(s->steer_cnt); free(s->in_collision);

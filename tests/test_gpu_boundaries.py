@@ -81,7 +81,7 @@ def tick_vs_oracle(f110, dev, dmap, poses, B=1080, fov=4.7, noise_std=0.0, omaps
     import philox_ref
     N, A = poses.shape[:2]
     sim = f110.Simulator(f110.maps.DEFAULT_PARAMS, A, 12345, num_envs=N, num_beams=B, fov=fov, device=dev,
-                         noise_std=noise_std, count_lookups=noise_std == 0.0)
+                         noise_std=noise_std, count_lookups=noise_std == 0.0, theta_dis=int(dmap.c.theta_dis))
     sim.set_device_map(dmap, env_map_ids=env_map_ids)
     sim.reset(poses)
     ids = np.zeros(N, int) if env_map_ids is None else np.asarray(env_map_ids)

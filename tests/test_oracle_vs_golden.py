@@ -292,6 +292,68 @@ def test_env_race2(example_map):
     assert done and sim.collisions[0] == 1.0 and np.array_equal(sim.lap_counts, [1.0, 1.0])
 
 
+CONFIG_MAPS = {'example_map': '.png', 'berlin': '.png'}
+
+
+@pytest.mark.parametrize('name', sorted(CONFIG_MAPS))
+def test_scans_off_default_config(name):
+    """ScanSimulator2D(B, fov, eps=, theta_dis=, max_range=) off the defaults (tests/golden/make_golden_configs.py): theta_dis
+    1000 / 4000 / 32767, max_range 5 / 40, eps 0.01, fov 0.1 / pi / 6.28 / 7.0 and B 2 / 3 / 33 / 100 / 8224, bit for bit."""
+    k = g('kat_configs.npz')
+    poses = k['poses_' + name]
+    hits = {}
+    for j, (B, fov, eps, td, mr) in enumerate(k['configs']):
+        B, td = int(B), int(td)
+        m = oracle.OracleMap.from_yaml(os.path.join(MAPS, name + '.yaml'), CONFIG_MAPS[name], theta_dis=td, eps=eps,
+                                       max_range=mr)
+        ref = k['scan_%d_%s' % (j, name)]
+        for p, want in zip(poses[:ref.shape[0]], ref):
+            got = oracle.get_scan(m, p, B, fov)
+            assert np.array_equal(got, want), (str(k['names'][j]), p)
+        hits[str(k['names'][j])] = int((ref == mr).sum())
+    # the 5 m clamp is reached more often than the default 30 m one, and that more often than the 40 m one
+    assert hits['mr5'] > hits['td1000'] >= hits['mr40'] and hits['mr5'] > 0, hits
+
+
+def test_env_ego1(example_map):
+    """F110Env(ego_idx=1) of the reference (tests/golden/env_ego1.npz): the ego's wall crash ends the episode; agent 0's
+    wall crash does not, and the lap toggles of both cars run in the ego's start frame."""
+    k = g('env_ego1.npz')
+    for ep, ego_crash in (('ego_crash_', True), ('opp_crash_', False)):
+        sim = oracle.OracleSim(example_map, num_agents=2, ego_idx=1)
+        done = sim.env_reset(k[ep + 'pose0'])
+        T = k[ep + 'actions'].shape[0]
+        for t in range(T):
+            if t > 0:
+                sim.step(k[ep + 'actions'][t])
+                done = sim.env_post_step()
+            assert np.array_equal(sim.state, k[ep + 'states'][t]), (ep, t)
+            assert np.array_equal(sim.collisions, k[ep + 'collisions'][t]), (ep, t)
+            assert np.array_equal(sim.lap_times, k[ep + 'lap_times'][t]), (ep, t)
+            assert np.array_equal(sim.lap_counts, k[ep + 'lap_counts'][t]), (ep, t)
+            assert np.array_equal(sim.toggle_list, k[ep + 'toggles'][t]), (ep, t)
+            assert done == bool(k[ep + 'done'][t]), (ep, t)
+        if ego_crash:
+            assert done and np.array_equal(sim.collisions, [0.0, 1.0])
+        else:
+            assert not done and np.array_equal(sim.collisions, [1.0, 0.0]) and sim.toggle_list.any()
+    # with the default ego (agent 0) the same actions end the second episode at agent 0's crash
+    sim = oracle.OracleSim(example_map, num_agents=2)
+    sim.env_reset(k['opp_crash_pose0'])
+    ends = []
+    for t in range(1, k['opp_crash_actions'].shape[0]):
+        sim.step(k['opp_crash_actions'][t])
+        ends.append(sim.env_post_step())
+    assert any(ends)
+
+
+def test_oracle_ego_idx_range(example_map):
+    with pytest.raises(ValueError):
+        oracle.OracleSim(example_map, num_agents=2, ego_idx=2)
+    with pytest.raises(ValueError):
+        oracle.OracleSim(example_map, num_agents=2, ego_idx=-1)
+
+
 def test_planner_vs_reference():
     """oracle pure pursuit == reference PurePursuitPlanner.plan (examples/waypoint_follow.py) incl. the
     re-acquire and no-waypoint branches; ulp-level slack for the BLAS dot products in the reference."""
