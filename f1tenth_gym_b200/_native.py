@@ -76,6 +76,12 @@ class F110Progress(C.Structure):
                 ('back', C.c_int32), ('fwd', C.c_int32), ('reacquire_dist', C.c_double)]
 
 
+class F110Repeat(C.Structure):
+    _fields_ = [('done_any', _dp), ('done_tick', _dp), ('list', _dp), ('list_count', _dp), ('marched_agents', _dp)]
+
+
+MAX_REPEAT = 64
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol declared
 # in include/f110_b200.h is exported.
 _P = C.POINTER
@@ -98,6 +104,10 @@ SIGNATURES = {
                             C.c_uint64, _dp]),
     'f110_tick_ex': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32, _dp, C.c_int32,
                                C.c_int32, C.c_uint64, _dp]),
+    'f110_tick_repeat': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32, _P(F110Repeat),
+                                   C.c_int32, _dp, C.c_int32, C.c_int32, C.c_uint64, _dp]),
+    'f110_tick_repeat_ticks': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32, C.c_int32,
+                                         C.c_int32, _P(F110Repeat), C.c_int32, _dp, C.c_int32, C.c_int32, C.c_uint64, _dp]),
     'f110_step_host': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs), _dp]),
     'f110_step_host_async': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs),
                                        _P(F110HostObs), _dp, _dp, _dp, _dp]),
@@ -121,6 +131,7 @@ SIGNATURES = {
                                            C.c_double, C.c_double, C.c_double, _dp, _dp]),
     'f110_track_project': (C.c_int, [_P(F110Track), _dp, _dp, C.c_int32, _dp, _dp]),
     'f110_track_progress': (C.c_int, [_P(F110Sim), _P(F110Track), _P(F110Progress), _dp]),
+    'f110_track_progress_sum': (C.c_int, [_P(F110Sim), _P(F110Track), _P(F110Progress), _dp, C.c_int32, _dp]),
     'f110_edt': (C.c_int, [_dp, C.c_int32, C.c_int32, C.c_double, _dp, _dp, _dp, _dp]),
     'f110_rasterize_track': (C.c_int, [_dp, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_int32, _dp, _dp, _dp]),
     'f110_scan_noise': (C.c_int, [_dp, C.c_int64, C.c_double, C.c_uint64, C.c_uint64, _dp]),

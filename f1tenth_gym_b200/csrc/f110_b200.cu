@@ -12,6 +12,8 @@
 //   k_tail         warp per agent       GJK vs. the other agents of the env, wall-hit state zeroing, opponent ray-cast inside the
 //                                       blocked-view window, collisions obs, then lap logic and auto-reset per env
 //                                       (k_finalize = the same without the env-level part, for f110_step)
+// f110_tick_repeat holds one action for K ticks: the last is the tick above, the others run k_dynamics, k_ttc_select, k_march_ttc
+// (march_ttc.cuh: only the agents a wall could stop, for the iTTC flag alone) and k_tail_noscan.
 // Host side of a tick (step_impl): validate -> classify_map (MapGeom: the map-geometry rules, shared with f110_scan_layers and
 // f110_render_views) -> plan_march (MarchPlan: kernel family, block shape, queue sizing; the only reader of the debug variant)
 // -> k_dynamics -> launch_march_plan (a switch on the family) -> launch_tail -> the launch record, written from the plan.
@@ -33,6 +35,7 @@
 #include "march_het.cuh"
 #include "march_rot.cuh"
 #include "scan_lean.cuh"
+#include "march_ttc.cuh"
 #include "render.cuh"
 #include "march_tile.cuh"
 #include "planner.cuh"
@@ -877,6 +880,83 @@ __global__ void __launch_bounds__(F110_TAIL2_THREADS, 3) k_tail2(f110_sim s, Bea
     if (blockIdx.x == 0 && threadIdx.x == 0) end_of_tick_housekeeping(s);
 }
 
+// ------------------------------------------------------------------------------------ k_tail_noscan (f110_tick_repeat)
+// The tail of a tick whose scans are withheld (march_ttc.cuh): k_tail2 without its task records and its phase 2, the opponent
+// ray-cast, which is the only part of a tail that touches scans.  A block owns whole envs (A <= 32): one thread per agent does
+// agent_duties, then one thread per env the lap logic, the done bookkeeping of the repeat call and the auto-reset.
+// The per-agent duties of a tail that one thread can do: wall-hit zeroing, GJK against the other agents of the env
+// (collision_multiple :184-212) and the collisions observation.  pa = the agent's pose snapshot.  The statements of k_tail2's
+// phase 1, kept apart from it: calling this from k_tail2 changes that kernel's code.
+__device__ __forceinline__ void agent_duties(const f110_sim &s, int env, int slot, int a, int hit, const double *pa) {
+    const int A = s.num_agents, NA = s.num_envs * A;
+    if (hit) {
+#pragma unroll
+        for (int q = 0; q < 4; q++) s.state[(size_t)(3 + q) * NA + a] = 0.0;
+    }
+    int col = 0, cidx = -1;
+    const double reach2 = (s.sim_length * s.sim_length + s.sim_width * s.sim_width) * 1.001;
+    for (int jj = 0; jj < A; jj++) {
+        if (jj == slot) continue;
+        const double *pc = s.agent_poses + 5 * (size_t)(env * A + jj);
+        const double ddx = pc[0] - pa[0], ddy = pc[1] - pa[1];
+        if (ddx * ddx + ddy * ddy > reach2) continue;
+        double vme[8], vo[8];
+        get_vertices_cs(pa[0], pa[1], pa[3], pa[4], s.sim_length, s.sim_width, vme);
+        get_vertices_cs(pc[0], pc[1], pc[3], pc[4], s.sim_length, s.sim_width, vo);
+        const bool c = (slot < jj) ? gjk_collision(vme, vo) : gjk_collision(vo, vme);
+        if (c) { col = 1; cidx = max(cidx, jj); }
+    }
+    s.collisions[a] = (col || hit) ? 1.0 : 0.0;
+    s.collision_idx[a] = cidx;
+}
+
+struct RepeatDone {
+    uint8_t *done_any;       // [N] or NULL
+    int32_t *done_tick;      // [N] or NULL
+    int tick;                // index of this tick inside the call
+};
+// done_any / done_tick of f110_repeat from this tick's done flag: tick 0 overwrites what the previous call left
+__device__ __forceinline__ void repeat_done_one(const f110_sim &s, int env, const RepeatDone &rd) {
+    const int d = s.done[env] ? 1 : 0;
+    if (rd.done_any) rd.done_any[env] = (uint8_t)((rd.tick == 0 ? 0 : rd.done_any[env]) | d);
+    if (rd.done_tick) {
+        const int first = rd.tick == 0 ? -1 : rd.done_tick[env];
+        rd.done_tick[env] = (first < 0 && d) ? rd.tick : first;
+    }
+}
+// after the ordinary tail of a tick of the call (its last one, or any tick of a call that takes the plain path)
+__global__ void k_repeat_done(f110_sim s, RepeatDone rd) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env < s.num_envs) repeat_done_one(s, env, rd);
+}
+
+__global__ void __launch_bounds__(F110_TAIL_NOSCAN_THREADS) k_tail_noscan(f110_sim s, int env_level, AutoResetArgs ar,
+                                                                          int envs_per_block, RepeatDone rd) {
+    const int A = s.num_agents;
+    const int env0 = blockIdx.x * envs_per_block;
+    const int envs_here = min(envs_per_block, s.num_envs - env0);
+    for (int la = threadIdx.x; la < envs_here * A; la += blockDim.x) {
+        const int envl = la / A, slot = la - envl * A;
+        const int a = env0 * A + la;
+        agent_duties(s, env0 + envl, slot, a, s.wall_flag[a], s.agent_poses + 5 * (size_t)a);
+    }
+    __syncthreads();
+    if ((int)threadIdx.x < envs_here) {
+        const int env = env0 + (int)threadIdx.x;
+        if (env_level) {
+            env_post_step_one(s, env);
+            repeat_done_one(s, env, rd);
+        }
+        if (ar.start_poses) autoreset_one(s, env, ar);
+    }
+}
+
+// f110_track_progress_sum: the deltas of the ticks of one policy step, summed in tick order
+__global__ void k_delta_sum(const double *__restrict__ delta, double *__restrict__ sum, int n, int restart) {
+    const int a = blockIdx.x * blockDim.x + threadIdx.x;
+    if (a < n) sum[a] = restart ? delta[a] : sum[a] + delta[a];
+}
+
 // ------------------------------------------------------------------------------------ standalone kernels
 __global__ void k_rhs(const double *__restrict__ x, const double *__restrict__ u, const double *__restrict__ p,
                       int M, double *__restrict__ f) {
@@ -1035,7 +1115,7 @@ static int check_beams(const f110_beams *b) {
 static unsigned long long *g_trace = nullptr;          // debug only: per-block timeline buffer (f110_debug_set_trace)
 static unsigned long long *g_tile_counter = nullptr;   // debug only: lookups served from the shared-memory tile
 // debug record of the kernels the last tick / f110_scan_layers of this thread launched (f110_debug_last_launch): host-side text only
-static thread_local char g_launch_rec[384] = "";
+static thread_local char g_launch_rec[448] = "";
 
 static int num_sms() {
     static int n = 0;
@@ -1883,6 +1963,149 @@ static void write_launch_record(const MarchPlan &p, const MapGeom &geom, const f
              p.rot && p.lean ? "" : " ROT=0", p.mq.static_runs, p.per_warp, tail);
 }
 
+// ------------------------------------------------------------------------------------ the plan and the launches of a tick
+struct TickPlan {
+    MapGeom geom;
+    MarchPlan march;
+};
+static int plan_tick(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                     const double *actions, TickPlan *tp) {
+    int rc;
+    if ((rc = check_sim(sim)) || (rc = check_map(map)) || (rc = check_beams(beams))) return rc;
+    if (!actions) return F110_ERR_INVALID;
+    if (sim->lookup_counter && sim->noise_std > 0.0) return F110_ERR_INVALID;   // counting runs are noise-free by construction
+    if ((long long)sim->num_envs * sim->num_agents > 0x7fffffffll) return F110_ERR_INVALID;
+    if ((rc = classify_map(map, &tp->geom))) return rc;
+    return plan_march(sim, map, tables, beams, tp->geom, rm_variant(), &tp->march);
+}
+static int launch_tick(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                       const double *actions, TickPlan &tp, cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail) {
+    int rc;
+    MarchPlan &plan = tp.march;
+    const bool pdl = (ev == nullptr);         // PDL only when no events are recorded between the kernels
+
+    if (ev) CUDA_TRY(cudaEventRecord(ev[0], st));
+    k_dynamics<<<plan.dyn_blocks + plan.order_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, plan.dyn_blocks,
+                                                                    fill_first_lookup(sim, map, beams, tp.geom, plan));
+    LAUNCH_CHECK("k_dynamics");
+    if (ev) CUDA_TRY(cudaEventRecord(ev[1], st));
+    if ((rc = launch_march_plan(plan, sim, map, tables, beams, tp.geom, pdl, st))) return rc;
+    if (ev) CUDA_TRY(cudaEventRecord(ev[2], st));
+    TailShape ts = {};
+    if ((rc = launch_tail(sim, map, make_view(beams), tail, pdl && plan.lean, st, &ts))) return rc;
+    write_launch_record(plan, tp.geom, map, ts);
+    if (ev) CUDA_TRY(cudaEventRecord(ev[3], st));
+    return F110_OK;
+}
+// ---- f110_tick_repeat: `repeat` ticks under one action; the ticks whose scans nobody reads march only for the iTTC flag
+// The plan of the call: the plain tick's plan, and whether ticks 0 .. repeat - 2 take the short path (march_ttc.cuh).  Decided
+// here from what the host can observe, never by an option.  The short path needs: no scan noise (the bound does not hold for
+// a Gaussian, and the Philox stream must stay the plain run's); a lean march family, which brings the per-agent record, the
+// doubled LUT and `dt_min_positive > eps`; a known max side distance below max_range (otherwise every moving agent is
+// listed); and at most 32 agents per env (the block-owns-envs tail).  Everything else runs `repeat` plain ticks.
+struct RepeatPlan {
+    TickPlan tick;
+    bool ttc;                // ticks 0 .. repeat - 2: k_dynamics, k_ttc_select, k_march_ttc, k_tail_noscan
+    int units;               // F110_SCAN_UNITS_* of k_march_ttc
+    unsigned grid;           // its fixed grid: resident blocks per SM x SMs
+};
+template <int UNITS>
+static int ttc_grid(bool count, unsigned *grid) {
+    static int per_sm[2] = {0, 0};
+    int &n = per_sm[count ? 1 : 0];
+    if (n <= 0) {
+        if (count) CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, true>, F110_TTC_THREADS, 0));
+        else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, false>, F110_TTC_THREADS, 0));
+        if (n <= 0) return F110_ERR_INVALID;
+    }
+    *grid = (unsigned)n * (unsigned)num_sms();
+    return F110_OK;
+}
+static int plan_repeat(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                       const double *actions, int32_t repeat, RepeatPlan *rp) {
+    int rc;
+    if ((rc = plan_tick(sim, map, tables, beams, actions, &rp->tick))) return rc;
+    const MarchPlan &m = rp->tick.march;
+    const bool lean_family = m.family == MarchFamily::LEAN || m.family == MarchFamily::LEAN_BRICK || m.family == MarchFamily::LEAN_HET ||
+                             m.family == MarchFamily::LEAN_HET_RES || m.family == MarchFamily::LEAN_ROT;
+    rp->ttc = repeat > 1 && sim->noise_std == 0.0 && m.lean && lean_family && sim->march_rec && map->sincos2 &&
+              map->dt_min_positive > map->eps && beams->side_max > 0.0 && beams->side_max < map->max_range && sim->num_agents <= 32;
+    rp->units = m.rot ? F110_SCAN_UNITS_ROT : m.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+    rp->grid = 0u;
+    if (!rp->ttc) return F110_OK;
+    const bool count = m.count;
+    return rp->units == F110_SCAN_UNITS_ROT ? ttc_grid<F110_SCAN_UNITS_ROT>(count, &rp->grid)
+         : rp->units == F110_SCAN_UNITS_CELLS ? ttc_grid<F110_SCAN_UNITS_CELLS>(count, &rp->grid)
+                                              : ttc_grid<F110_SCAN_UNITS_METRES>(count, &rp->grid);
+}
+
+static TtcK fill_ttc_k(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const RepeatPlan &rp, const f110_repeat *rep,
+                       int tick) {
+    const MarchPlan &m = rp.tick.march;
+    const bool het = rp.tick.geom.het;
+    TtcK q;
+    q.table = m.cell_units ? map->dt_cells_pad : map->dt;
+    q.dt = map->dt;
+    q.sincos2 = reinterpret_cast<const double2 *>(map->sincos2);
+    q.cos_side = reinterpret_cast<const double2 *>(beams->cos_side);
+    q.rec = reinterpret_cast<const double2 *>(sim->march_rec);
+    q.list = rep->list; q.count = rep->list_count + tick;
+    q.wall_flag = sim->wall_flag; q.lookup_counter = sim->lookup_counter;
+    q.layer_geom = het ? map->layer_geom : nullptr; q.layer_res = het ? map->layer_res : nullptr;
+    q.layer_rot = het ? map->layer_rot : nullptr; q.env_layer = het ? sim->env_layer : nullptr;
+    q.orig = make_double2(map->orig_x, map->orig_y);
+    q.ext = make_double2(map->width * map->resolution, map->height * map->resolution);
+    q.res = make_double2(map->resolution, 1.0 / map->resolution);
+    q.rot = make_double2(map->orig_c, map->orig_s);
+    q.tmax = m.cell_units ? map->max_range * (1.0 / map->resolution) : map->max_range;
+    q.max_range = map->max_range; q.eps = map->eps;
+    q.ttc_thresh = sim->ttc_thresh; q.ttc_margin = sim->ttc_thresh * 1.000001;
+    q.inc = beams->theta_index_increment; q.theta_dis_f = (double)map->theta_dis;
+    lut_fixed_point(beams, &q.inc_fx, &q.guard32);
+    q.layer_stride = (unsigned long long)map->width * (unsigned long long)map->height;
+    q.layer_stride_lean = m.cell_units ? (unsigned long long)(map->width + 1) * (unsigned long long)(map->height + 1) : q.layer_stride;
+    q.width = (unsigned)map->width; q.height = (unsigned)map->height;
+    q.last = (unsigned)map->width * (unsigned)map->height - 1u;
+    q.ipa = (unsigned)((beams->num_beams + 31) / 32);
+    q.num_agents = (unsigned)sim->num_agents;
+    q.B = beams->num_beams;
+    return q;
+}
+
+template <int UNITS>
+static void launch_march_ttc_t(const TtcK &q, bool count, unsigned grid, cudaStream_t st) {
+    if (count) k_march_ttc<UNITS, true><<<grid, F110_TTC_THREADS, 0, st>>>(q);
+    else k_march_ttc<UNITS, false><<<grid, F110_TTC_THREADS, 0, st>>>(q);
+}
+
+// one intermediate tick of the short path
+static int launch_ttc_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
+                           const RepeatPlan &rp, const f110_repeat *rep, int tick, const TailOpts &tail, cudaStream_t st) {
+    const MarchPlan &m = rp.tick.march;
+    const int NA = sim->num_envs * sim->num_agents;
+    // k_dynamics without its queue-building blocks: the queue is built once, by the last tick of the call
+    k_dynamics<<<m.dyn_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, m.dyn_blocks,
+                                             fill_first_lookup(sim, map, beams, rp.tick.geom, m));
+    LAUNCH_CHECK("k_dynamics");
+    TtcSelectK sel;
+    sel.rec = reinterpret_cast<const double2 *>(sim->march_rec); sel.list = rep->list; sel.count = rep->list_count + tick;
+    sel.marched = rep->marched_agents; sel.d0_scale = m.cell_units ? map->resolution : 1.0; sel.max_range = map->max_range;
+    sel.agents = (unsigned)NA;
+    k_ttc_select<<<(NA + F110_TTC_SELECT_THREADS - 1) / F110_TTC_SELECT_THREADS, F110_TTC_SELECT_THREADS, 0, st>>>(sel);
+    LAUNCH_CHECK("k_ttc_select");
+    const TtcK q = fill_ttc_k(sim, map, beams, rp, rep, tick);
+    if (rp.units == F110_SCAN_UNITS_ROT) launch_march_ttc_t<F110_SCAN_UNITS_ROT>(q, m.count, rp.grid, st);
+    else if (rp.units == F110_SCAN_UNITS_CELLS) launch_march_ttc_t<F110_SCAN_UNITS_CELLS>(q, m.count, rp.grid, st);
+    else launch_march_ttc_t<F110_SCAN_UNITS_METRES>(q, m.count, rp.grid, st);
+    LAUNCH_CHECK("k_march_ttc");
+    const int epb = std::max(1, F110_TAIL_NOSCAN_THREADS / sim->num_agents);
+    RepeatDone rd;
+    rd.done_any = rep->done_any; rd.done_tick = rep->done_tick; rd.tick = tick;
+    k_tail_noscan<<<(sim->num_envs + epb - 1) / epb, F110_TAIL_NOSCAN_THREADS, 0, st>>>(*sim, (int)tail.env_level, tail.ar, epb, rd);
+    LAUNCH_CHECK("k_tail_noscan");
+    return F110_OK;
+}
+
 }  // namespace f110
 
 using namespace f110;
@@ -1948,28 +2171,10 @@ const char *f110_last_cuda_error(void) { return g_cuda_err; }
 static int step_impl(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                      const double *actions, cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail = nullptr) {
     int rc;
-    if ((rc = check_sim(sim)) || (rc = check_map(map)) || (rc = check_beams(beams))) return rc;
-    if (!actions) return F110_ERR_INVALID;
-    if (sim->lookup_counter && sim->noise_std > 0.0) return F110_ERR_INVALID;   // counting runs are noise-free by construction
-    if ((long long)sim->num_envs * sim->num_agents > 0x7fffffffll) return F110_ERR_INVALID;
     g_launch_rec[0] = '\0';
-    MapGeom geom;
-    MarchPlan plan;
-    if ((rc = classify_map(map, &geom)) || (rc = plan_march(sim, map, tables, beams, geom, rm_variant(), &plan))) return rc;
-    const bool pdl = (ev == nullptr);         // PDL only when no events are recorded between the kernels
-
-    if (ev) CUDA_TRY(cudaEventRecord(ev[0], st));
-    k_dynamics<<<plan.dyn_blocks + plan.order_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, plan.dyn_blocks,
-                                                                    fill_first_lookup(sim, map, beams, geom, plan));
-    LAUNCH_CHECK("k_dynamics");
-    if (ev) CUDA_TRY(cudaEventRecord(ev[1], st));
-    if ((rc = launch_march_plan(plan, sim, map, tables, beams, geom, pdl, st))) return rc;
-    if (ev) CUDA_TRY(cudaEventRecord(ev[2], st));
-    TailShape ts = {};
-    if ((rc = launch_tail(sim, map, make_view(beams), tail, pdl && plan.lean, st, &ts))) return rc;
-    write_launch_record(plan, geom, map, ts);
-    if (ev) CUDA_TRY(cudaEventRecord(ev[3], st));
-    return F110_OK;
+    TickPlan tp;
+    if ((rc = plan_tick(sim, map, tables, beams, actions, &tp))) return rc;
+    return launch_tick(sim, map, tables, beams, actions, tp, st, ev, tail);
 }
 
 int f110_step(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
@@ -2073,21 +2278,74 @@ int f110_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams,
               void *stream) {
     return f110_tick_ex(sim, map, nullptr, beams, actions, env_level, start_poses, num_start, pose_gap, seed, stream);
 }
-int f110_tick_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
-                 const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
-                 uint64_t seed, void *stream) {
+// the checks and the tail options of a whole tick (f110_tick_ex, f110_tick_repeat)
+static int tick_tail_opts(const f110_sim *sim, const f110_map *map, int32_t env_level, const double *start_poses, int32_t num_start,
+                          int32_t pose_gap, uint64_t seed, TailOpts *t) {
     int rc;
     if ((rc = check_sim(sim))) return rc;
     if (env_level && (rc = check_env_arrays(sim))) return rc;
     if (start_poses && (num_start <= 0 || sim->ego_idx < 0 || sim->ego_idx >= sim->num_agents || sim->num_agents > 32))
         return F110_ERR_INVALID;
+    t->fused = true; t->env_level = env_level;
+    t->ar.start_poses = start_poses; t->ar.num_start = num_start; t->ar.pose_gap = pose_gap; t->ar.seed = seed; t->ar.tick_host = 0;
+    t->ar.num_tables = 0;
+    if (start_poses && (rc = start_tables(sim, num_start, t->ar))) return rc;
+    if (t->ar.num_tables && (!map || t->ar.num_tables != map->num_layers)) return F110_ERR_INVALID;
+    return F110_OK;
+}
+
+int f110_tick_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                 const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                 uint64_t seed, void *stream) {
+    int rc;
     TailOpts t;
-    t.fused = true; t.env_level = env_level;
-    t.ar.start_poses = start_poses; t.ar.num_start = num_start; t.ar.pose_gap = pose_gap; t.ar.seed = seed; t.ar.tick_host = 0;
-    t.ar.num_tables = 0;
-    if (start_poses && (rc = start_tables(sim, num_start, t.ar))) return rc;
-    if (t.ar.num_tables && (!map || t.ar.num_tables != map->num_layers)) return F110_ERR_INVALID;
+    if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
     return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, &t);
+}
+
+int f110_tick_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                           const double *actions, int32_t repeat, int32_t first_tick, int32_t num_ticks, const f110_repeat *rep,
+                           int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
+                           void *stream) {
+    int rc;
+    TailOpts t;
+    RepeatPlan rp;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
+    if (repeat < 1 || repeat > F110_MAX_REPEAT || first_tick < 0 || num_ticks < 1 || first_tick > repeat - num_ticks) return F110_ERR_INVALID;
+    if (!rep || !rep->list || !rep->list_count) return F110_ERR_INVALID;
+    if ((rep->done_any || rep->done_tick) && !env_level) return F110_ERR_INVALID;     // done is computed by the env-level part
+    g_launch_rec[0] = '\0';
+    if ((rc = plan_repeat(sim, map, tables, beams, actions, repeat, &rp))) return rc;
+
+    if (first_tick == 0) CUDA_TRY(cudaMemsetAsync(rep->list_count, 0, sizeof(uint32_t) * (size_t)repeat, st));
+    const bool track_done = rep->done_any || rep->done_tick;
+    for (int tick = first_tick; tick < first_tick + num_ticks; tick++) {
+        if (rp.ttc && tick < repeat - 1) {
+            if ((rc = launch_ttc_tick(sim, map, beams, actions, rp, rep, tick, t, st))) return rc;
+            continue;
+        }
+        if ((rc = launch_tick(sim, map, tables, beams, actions, rp.tick, st, nullptr, &t))) return rc;
+        if (track_done) {
+            RepeatDone rd;
+            rd.done_any = rep->done_any; rd.done_tick = rep->done_tick; rd.tick = tick;
+            k_repeat_done<<<(sim->num_envs + 127) / 128, 128, 0, st>>>(*sim, rd);
+            LAUNCH_CHECK("k_repeat_done");
+        }
+    }
+    // the record of the call: the last plain tick's record (when the range holds one) and the repeat part
+    const size_t n = strlen(g_launch_rec);
+    static const char *units[3] = {"cells", "metres", "rot"};
+    snprintf(g_launch_rec + n, sizeof(g_launch_rec) - n, "%srepeat=%d sub=%s UNITS=%s grid=%u", n ? " " : "", (int)repeat,
+             rp.ttc ? "ttc" : "full", units[rp.units], rp.grid);
+    return F110_OK;
+}
+
+int f110_tick_repeat(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                     const double *actions, int32_t repeat, const f110_repeat *rep, int32_t env_level, const double *start_poses,
+                     int32_t num_start, int32_t pose_gap, uint64_t seed, void *stream) {
+    return f110_tick_repeat_ticks(sim, map, tables, beams, actions, repeat, 0, repeat, rep, env_level, start_poses, num_start,
+                                  pose_gap, seed, stream);
 }
 
 int f110_step_host(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions_host,
@@ -2449,6 +2707,17 @@ int f110_track_progress(const f110_sim *sim, const f110_track *track, f110_progr
     p.back = g.back; p.window = g.back + g.fwd + 1;
     k_track_progress<<<(unsigned)(((long long)p.NA * 32 + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
     LAUNCH_CHECK("k_track_progress");
+    return F110_OK;
+}
+
+int f110_track_progress_sum(const f110_sim *sim, const f110_track *track, f110_progress *progress, double *delta_sum,
+                            int32_t restart, void *stream) {
+    int rc;
+    if (!delta_sum) return F110_ERR_INVALID;
+    if ((rc = f110_track_progress(sim, track, progress, stream))) return rc;
+    const int NA = sim->num_envs * sim->num_agents;
+    k_delta_sum<<<(NA + 255) / 256, 256, 0, (cudaStream_t)stream>>>(progress->delta, delta_sum, NA, restart);
+    LAUNCH_CHECK("k_delta_sum");
     return F110_OK;
 }
 

@@ -18,6 +18,10 @@ obs['track_heading_error'] and obs['progress'] ((N, A) device tensors in batched
 after every step on the device; reward='progress' (needs centerline) returns the ego's progress along its centerline in that
 step, (N,) on the device (a copy, still valid after the next step) or a float, instead of the reference's constant timestep.
 An env reset since its last step restarts its progress at 0, so the step that resets an env earns 0.
+action_repeat=K (default 1): step() holds the action for K ticks (Simulator.tick_repeat, one call).  done is then "done on any
+of the K ticks" and info['done_tick'] the first such tick (-1: none); the reward is K * timestep, or with reward='progress' the
+sum of the ego's K deltas; lap_times, lap_counts, the progress keys and the scans are the last tick's.  The only difference to
+calling step() K times is which scans exist.  reset() still runs exactly one zero-action tick.
 Batched mode also takes a list of maps, map=['berlin', 'vegas', ...] with map_ext one extension or a list, stacked into
 one simulator (DeviceMap.stack: one resolution, unrotated origins); env e drives on map env_map_ids[e] (default e % L).
 mixed_resolution=True also stacks maps of different resolutions (e.g. generated tracks with the bundled maps); every map
@@ -80,6 +84,10 @@ class F110Env(object):
         self.centerline = kwargs.get('centerline', None)
         if self.reward_kind == 'progress' and self.centerline is None:
             raise ValueError("reward='progress' needs centerline=")
+        self.action_repeat = kwargs.get('action_repeat', 1)
+        if int(self.action_repeat) != self.action_repeat or not 1 <= self.action_repeat <= 64:
+            raise ValueError('action_repeat must be an int in [1, 64], got %r' % (self.action_repeat,))
+        self.action_repeat = int(self.action_repeat)
         self._set_map(self.map_path, self.map_ext)
         self.render_obs = None
         self._local_map_buf = None
@@ -179,18 +187,49 @@ class F110Env(object):
         return o, reward, bool(io['done'].numpy()[0]), {'checkpoint_done': lap_counts >= 2}
 
     def step(self, action):
-        """f110_env.py:263-304."""
+        """f110_env.py:263-304; with action_repeat=K, K ticks under `action` (see the module text)."""
+        if self.action_repeat > 1:
+            return self._step_repeat(action)
         if not self.batched:
             return self._step_single(action)
         obs = self.sim.step(action)
         return self._finish(obs)
+
+    def _step_repeat(self, action):
+        sim, K, N, A = self.sim, self.action_repeat, self.num_envs, self.num_agents
+        tracked = self.centerline is not None
+        a = action if torch.is_tensor(action) else np.asarray(action, dtype=np.float64).reshape(N, A, 2)
+        obs = sim.tick_repeat(a, K, env_level=True, progress=tracked)
+        obs['lap_times'], obs['lap_counts'] = sim.lap_times.view(N, A), sim.lap_counts.view(N, A)
+        if self._local_map is not None:
+            obs['local_map'] = self._render_local_map()
+        reward = K * self.timestep
+        if tracked:
+            for k, v in PROGRESS_KEYS:
+                obs[k] = sim._progress_views[v]
+            if self.reward_kind == 'progress':
+                reward = sim.track_delta_sum.view(N, A)[:, self.ego_idx].clone()
+        done, done_tick = obs.pop('done_any').bool(), obs.pop('done_tick')
+        info = {'checkpoint_done': sim.checkpoint_done.view(N, A).bool(), 'done_tick': done_tick}
+        if self.batched:
+            return obs, reward, done, info
+        # single env, reference-shaped: lists of per-agent values
+        o = {k: (v if k == 'ego_idx' else v[0].cpu().numpy()) for k, v in obs.items()}
+        o['scans'] = [s for s in o['scans'].astype(np.float64)]
+        for k in ('poses_x', 'poses_y', 'poses_theta', 'linear_vels_x', 'linear_vels_y', 'ang_vels_z'):
+            o[k] = [float(v) for v in o[k]]
+        reward = float(reward[0].item()) if torch.is_tensor(reward) else reward
+        return o, reward, bool(done[0].item()), {'checkpoint_done': info['checkpoint_done'][0].cpu().numpy(),
+                                                'done_tick': int(done_tick[0].item())}
 
     def reset(self, poses):
         """f110_env.py:306-349: zero counters, start frame, Simulator.reset, then ONE zero-action tick
         whose (obs, reward, done, info) is returned."""
         self.sim.env_reset(poses)
         action = torch.zeros((self.num_envs, self.num_agents, 2), dtype=torch.float64, device=self.sim.device)
-        return self.step(action)
+        if not self.batched:
+            return self._step_single(action)
+        return self._finish(self.sim.step(action))
 
     def reset_envs(self, env_mask, poses):
         """Batch extension: re-initialise only the masked envs (counters + Simulator.reset); no tick is run."""

@@ -404,6 +404,12 @@ class Simulator(object):
         self.centerlines = None
         self.track_seg = self.track_s = self.track_d = self.track_heading_error = None
         self.track_progress = self.track_delta = None
+        # outputs and scratch of tick_repeat (C ABI f110_repeat), allocated on first use
+        self.done_any = self.done_tick = self.repeat_list = self.repeat_list_count = self.marched_agents = None
+        self.track_delta_sum = None
+        self._repeat_c = None
+        self._repeat_ticks = 0      # intermediate agent-ticks issued since the counter was last read (marched_fraction)
+        self._repeat_plain = False
 
     # ------------------------------------------------------------------ configuration
     def set_map(self, map_path, map_ext, edt='scipy'):
@@ -581,6 +587,81 @@ class Simulator(object):
                                          int(seed), _stream_ptr(self.device)))
         return self.observations()
 
+    def _repeat_struct(self):
+        """The f110_repeat outputs and scratch, allocated once."""
+        if self._repeat_c is None:
+            N, NA, dev = self.num_envs, self.num_envs * self.num_agents, self.device
+            self.done_any = torch.zeros((N,), dtype=torch.uint8, device=dev)
+            self.done_tick = torch.full((N,), -1, dtype=torch.int32, device=dev)
+            self.repeat_list = torch.zeros((NA,), dtype=torch.int32, device=dev)
+            self.repeat_list_count = torch.zeros((nat.MAX_REPEAT,), dtype=torch.int32, device=dev)
+            self.marched_agents = torch.zeros((1,), dtype=torch.int64, device=dev)
+            self._repeat_c = nat.F110Repeat(nat.ptr(self.done_any), nat.ptr(self.done_tick), nat.ptr(self.repeat_list),
+                                            nat.ptr(self.repeat_list_count), nat.ptr(self.marched_agents))
+        return self._repeat_c
+
+    def _check_repeat(self, repeat):
+        if int(repeat) != repeat or not 1 <= int(repeat) <= nat.MAX_REPEAT:
+            raise ValueError('repeat must be an int in [1, %d], got %r' % (nat.MAX_REPEAT, repeat))
+        return int(repeat)
+
+    def _issue_repeat(self, L, actions, K, call, env_level, table, num_start, pose_gap, seed, progress):
+        """Enqueue one f110_tick_repeat call; progress: the tracker is updated after every tick of the call (the same ticks,
+        issued one by one) and track_delta_sum gets the sum of the call's deltas."""
+        def ticks(first, count):
+            nat.check(L.f110_tick_repeat_ticks(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                               C.byref(self.beams.c), nat.ptr(actions), K, first, count, C.byref(call),
+                                               1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(seed),
+                                               _stream_ptr(self.device)))
+        if not progress:
+            ticks(0, K)
+            return
+        for t in range(K):
+            ticks(t, 1)
+            nat.check(L.f110_track_progress_sum(C.byref(self.c), C.byref(self.centerlines.c), C.byref(self._progress_c),
+                                                nat.ptr(self.track_delta_sum), 1 if t == 0 else 0, _stream_ptr(self.device)))
+
+    def _repeat_call(self, env_level, progress):
+        """The f110_repeat struct of a call (without the done outputs when the env level is off) after allocating what the
+        call writes."""
+        rep = self._repeat_struct()
+        if progress:
+            if self.centerlines is None:
+                raise ValueError('no centerlines: call set_centerlines first')
+            if self.track_delta_sum is None:
+                self.track_delta_sum = torch.zeros_like(self.track_delta)
+        return rep if env_level else nat.F110Repeat(None, None, rep.list, rep.list_count, rep.marched_agents)
+
+    def tick_repeat(self, control_inputs, repeat, env_level=True, autoreset_poses=None, pose_gap=23, seed=12345, progress=False):
+        """`repeat` ticks under one action in one call (C ABI f110_tick_repeat): everything except the scans is what `repeat`
+        calls of tick() leave, and the scans are the last tick's.  Returns observations() plus 'done_any' (N,) uint8, whether
+        an env was done on any tick of the call, and 'done_tick' (N,) int32, the first such tick or -1 (device views, overwritten
+        by the next call; both need env_level).  On the ticks before the last only the agents a wall could stop are marched.
+        progress=True (needs set_centerlines): update_progress() after every tick of the call; track_delta_sum (N*A,) then
+        holds each agent's progress over the whole call."""
+        K = self._check_repeat(repeat)
+        a = self._actions_tensor(control_inputs)
+        table, n = self._start_table(autoreset_poses)
+        call = self._repeat_call(env_level, progress)
+        self._issue_repeat(nat.lib(), a, K, call, env_level, table, n, pose_gap, seed, progress)
+        self._repeat_ticks += (K - 1) * self.num_envs * self.num_agents
+        self._repeat_plain = b'sub=full' in nat.lib().f110_debug_last_launch()      # the call ran plain ticks throughout
+        obs = self.observations()
+        if env_level:
+            obs['done_any'], obs['done_tick'] = self.done_any, self.done_tick
+        return obs
+
+    def marched_fraction(self):
+        """Share of the agent-ticks on the intermediate ticks of the tick_repeat calls since the last reading that had to be
+        ray-marched (1.0 when the calls ran plain ticks; None before any intermediate tick).  Synchronises the host: a
+        measurement, not for the hot loop.  Calls replayed from a captured graph are not counted."""
+        if self._repeat_ticks == 0:
+            return None
+        frac = 1.0 if self._repeat_plain else float(self.marched_agents.item()) / self._repeat_ticks
+        self.marched_agents.zero_()
+        self._repeat_ticks = 0
+        return frac
+
     def observations(self):
         N, A, B = self.num_envs, self.num_agents, self.num_beams
         st = self.state
@@ -602,6 +683,7 @@ class Simulator(object):
         count, back + fwd + 1 outside [1, 1024] or reacquire_dist not finite and > 0.  Every agent starts unacquired.
         None turns tracking off."""
         self._graph = None
+        self.track_delta_sum = None
         if tables is None:
             self.centerlines = None
             self.track_seg = self.track_s = self.track_d = self.track_heading_error = None
@@ -738,25 +820,33 @@ class Simulator(object):
 
     # ------------------------------------------------------------------ throughput paths
     def capture_graph(self, actions, autoreset_poses=None, pose_gap=23, autoreset_seed=12345, env_level=False,
-                      progress=False):
+                      progress=False, repeat=1):
         """Capture one tick (f110_step [+ env_post_step] [+ autoreset]) reading `actions` (a persistent
         device tensor the caller overwrites between replays) into a CUDA graph.  The warm-up tick that precedes the
         capture runs on a snapshot: every simulation buffer (state, FIFO, scans, lap counters, tick counter / noise
         stream, march queue history, progress tracker) is restored afterwards, so capturing has no side effect on the
-        simulation.  progress=True appends update_progress() to the captured tick (needs set_centerlines)."""
+        simulation.  progress=True appends update_progress() to the captured tick (needs set_centerlines).
+        repeat > 1 captures tick_repeat(actions, repeat) instead (done_any / done_tick with env_level); with progress=True the
+        tracker is updated after every tick of the call and track_delta_sum (N*A,) holds the sum of the call's deltas."""
         assert actions.is_cuda and actions.dtype == torch.float64 and actions.is_contiguous()
         if progress and self.centerlines is None:
             raise ValueError('capture_graph(progress=True) needs set_centerlines first')
         L = nat.lib()
+        K = self._check_repeat(repeat)
+        call = self._repeat_call(env_level, progress) if K > 1 else None
         names = ('state', 'steer_buf', 'steer_cnt', 'scan_pose', 'agent_poses', 'scans', 'wall_flag', 'collisions',
                  'collision_idx', 'current_time', 'lap_times', 'lap_counts', 'toggle_list', 'near_starts', 'start_xs',
                  'start_ys', 'start_thetas', 'start_rot', 'done', 'checkpoint_done', 'tick_counter', 'march_cost',
                  'march_order', 'march_count', 'march_rec', 'track_seg', 'track_s', 'track_d', 'track_heading_error',
-                 'track_progress', 'track_delta')
+                 'track_progress', 'track_delta', 'done_any', 'done_tick', 'repeat_list', 'repeat_list_count',
+                 'marched_agents', 'track_delta_sum')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
 
         def tick():
+            if K > 1:
+                self._issue_repeat(L, actions, K, call, env_level, table, num_start, pose_gap, autoreset_seed, progress)
+                return
             nat.check(L.f110_tick_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
                                      C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
                                      pose_gap, int(autoreset_seed), _stream_ptr(self.device)))
@@ -775,7 +865,8 @@ class Simulator(object):
         with torch.cuda.graph(g):
             tick()
         self._graph = g
-        self._graph_keep = (actions, table) + ((self.centerlines, self._progress_views) if progress else ())
+        self._graph_keep = (actions, table) + ((self.centerlines, self._progress_views) if progress else ()) + \
+            ((call,) if K > 1 else ())
         return g
 
     def replay(self):

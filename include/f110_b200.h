@@ -237,6 +237,48 @@ int f110_tick_ex(const f110_sim *sim, const f110_map *map, const f110_march_tabl
                  const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
                  uint64_t seed, void *stream);
 
+/* ---- action repeat: one action held for `repeat` ticks in one call ---- */
+#define F110_MAX_REPEAT 64
+/* Outputs and scratch of f110_tick_repeat, caller-owned device memory. */
+typedef struct {
+    uint8_t *done_any;                    /* [N] or NULL: OR of done[env] over the ticks of the call (overwritten, not accumulated) */
+    int32_t *done_tick;                   /* [N] or NULL: index 0..repeat-1 of the first tick of the call that set done, -1 = none */
+    uint32_t *list;                       /* [N*A] scratch: flat ids of the agents marched on an intermediate tick */
+    uint32_t *list_count;                 /* [repeat] scratch, zeroed by the call on `stream` */
+    unsigned long long *marched_agents;   /* [1] or NULL: += agents marched on intermediate ticks (measurement) */
+} f110_repeat;
+
+/* `repeat` whole ticks under one action (the "action repeat" / "frame skip" of a policy that runs slower than the physics):
+ * what `repeat` calls of f110_tick_ex with the same arguments do, except that only the LAST tick's scans exist.
+ *   - Enqueues everything on `stream`: no host synchronisation, no allocation, no global device state; capturable in a CUDA
+ *     graph.  1 <= repeat <= F110_MAX_REPEAT; that, `rep` or its two scratch pointers NULL, done_any / done_tick without
+ *     env_level, and everything f110_tick_ex rejects, return an error before anything is enqueued.
+ *   - After the call every buffer of f110_sim except scans, march_cost / march_order / march_count and *lookup_counter holds,
+ *     bit for bit, what the `repeat` plain ticks leave: state, steer FIFO and count (the FIFO sees the action once per tick),
+ *     scan_pose, agent_poses, march_rec, wall_flag, collisions, collision_idx, time, lap arrays, toggles, done,
+ *     checkpoint_done and tick_counter (advanced `repeat` times: the auto-reset draws and the noise stream are the plain
+ *     ticks').  scans holds the last tick's scans, bit-identical to the plain run's; between launches it is unspecified.
+ *   - An env that ends inside the call auto-resets on that tick (when start_poses is given) and keeps ticking in its new
+ *     episode under the same action, as the plain ticks do; done is the last tick's, done_any / done_tick report the
+ *     earlier ones.  repeat == 1 is f110_tick_ex plus done_any = done.
+ *   - On ticks 0 .. repeat-2 the reference's only remaining use of the scan is the iTTC wall check (laser_models.py:188-217).
+ *     An agent whose first distance-table lookup already exceeds the iTTC pre-test threshold of its speed cannot fire it and is
+ *     not marched at all; the others are marched for the flag alone (csrc/march_ttc.cuh).  That path is taken when the tick's
+ *     ray march is one of the lean kernels, the scan noise is off, beams->side_max is known and below max_range, and there
+ *     are at most 32 agents per env; otherwise every tick of the call is the plain tick and the contract above still holds.
+ *   - *lookup_counter counts the lookups actually performed.  The queue history (march_cost) is written by the last tick
+ *     alone, so its queue is ordered by costs that are `repeat` ticks old; results never depend on the queue. */
+int f110_tick_repeat(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                     const double *actions, int32_t repeat, const f110_repeat *rep, int32_t env_level,
+                     const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed, void *stream);
+/* Ticks first_tick .. first_tick + num_ticks - 1 of such a call, for a caller that has launches of its own to put between the
+ * ticks (f110_track_progress after every tick): issuing the ranges of one call in order, with the same arguments, is the
+ * call.  first_tick == 0 zeroes list_count.  F110_ERR_INVALID for a range outside [0, repeat). */
+int f110_tick_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                           const double *actions, int32_t repeat, int32_t first_tick, int32_t num_ticks, const f110_repeat *rep,
+                           int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
+                           void *stream);
+
 /* Same tick through HOST buffers: copies actions H2D, runs f110_step (+ f110_env_post_step when the
  * lap arrays are bound), copies the observation D2H and synchronises the stream.
  * Any output pointer may be NULL to skip that copy.  Host buffers should be pinned. */
@@ -404,6 +446,12 @@ int f110_track_project(const f110_track *track, const double *poses, const int32
  * pointers, no table, min_segments < 3, a bad window, reacquire_dist not finite or <= 0.  No global state, allocation or
  * host synchronisation: capturable in a CUDA graph after f110_tick.  Kernel k_track_progress (csrc/progress.cuh). */
 int f110_track_progress(const f110_sim *sim, const f110_track *track, f110_progress *progress, void *stream);
+
+/* f110_track_progress, then delta_sum[a] = (restart ? 0 : delta_sum[a]) + progress->delta[a] for every agent (delta_sum [N*A]
+ * fp64, device): the progress of a policy step that spans several ticks, summed in tick order (restart != 0 on its first tick).
+ * F110_ERR_INVALID for a NULL delta_sum and for what f110_track_progress rejects. */
+int f110_track_progress_sum(const f110_sim *sim, const f110_track *track, f110_progress *progress, double *delta_sum,
+                            int32_t restart, void *stream);
 
 /* Exact Euclidean distance transform on the device (load-time; reference laser_models.py:40-53 get_dt =
  * resolution * scipy.ndimage.distance_transform_edt(bitmap)): occupied [H][W] u8 (1 where the thresholded image
