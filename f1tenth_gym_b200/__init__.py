@@ -8,6 +8,7 @@ names).  Compute happens only in libf110_b200.so (hand-written sm_90a CUDA behin
 from .simulator import Integrator, Simulator, DeviceMap, DeviceBeams   # noqa: F401
 from .env import F110Env                                              # noqa: F401
 from . import kernels, maps, trackgen                                 # noqa: F401
+from .obstacles import obstacle_candidates                            # noqa: F401
 from .kernels import ScanSimulator2D                                  # noqa: F401
 from .planner import PurePursuitPlanner                               # noqa: F401
 

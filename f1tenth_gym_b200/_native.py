@@ -82,6 +82,15 @@ class F110Repeat(C.Structure):
 
 MAX_REPEAT = 64
 
+
+class F110Obstacles(C.Structure):
+    _fields_ = [('per_env', C.c_int32), ('boxes', _dp), ('active', _dp), ('hit', _dp), ('candidates', _dp),
+                ('cand_offsets', _dp), ('num_candidates', C.c_int32), ('num_cand_tables', C.c_int32),
+                ('count_min', C.c_int32), ('count_max', C.c_int32), ('clearance', C.c_double), ('seed', C.c_uint64)]
+
+
+MAX_OBSTACLES = 16
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol declared
 # in include/f110_b200.h is exported.
 _P = C.POINTER
@@ -108,6 +117,14 @@ SIGNATURES = {
                                    C.c_int32, _dp, C.c_int32, C.c_int32, C.c_uint64, _dp]),
     'f110_tick_repeat_ticks': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32, C.c_int32,
                                          C.c_int32, _P(F110Repeat), C.c_int32, _dp, C.c_int32, C.c_int32, C.c_uint64, _dp]),
+    'f110_step_obst': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, _P(F110Obstacles), _dp]),
+    'f110_tick_obst': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32, _dp, C.c_int32,
+                                 C.c_int32, C.c_uint64, _P(F110Obstacles), _dp]),
+    'f110_tick_repeat_ticks_obst': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32,
+                                              C.c_int32, C.c_int32, _P(F110Repeat), C.c_int32, _dp, C.c_int32, C.c_int32,
+                                              C.c_uint64, _P(F110Obstacles), _dp]),
+    'f110_autoreset_obst': (C.c_int, [_P(F110Sim), _dp, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _P(F110Obstacles), _dp]),
+    'f110_obstacles_respawn': (C.c_int, [_P(F110Sim), _P(F110Obstacles), _dp, C.c_uint64, _dp]),
     'f110_step_host': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs), _dp]),
     'f110_step_host_async': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs),
                                        _P(F110HostObs), _dp, _dp, _dp, _dp]),
@@ -117,6 +134,8 @@ SIGNATURES = {
     'f110_scan_layers': (C.c_int, [_P(F110Map), _P(F110Beams), _dp, _dp, C.c_int32, _dp, _dp, _dp, _dp]),
     'f110_render_views': (C.c_int, [_P(F110Sim), _P(F110Map), _dp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double,
                                     C.c_int32, _dp, _dp]),
+    'f110_render_views_obst': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Obstacles), _dp, C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_double, C.c_double, C.c_int32, _dp, _dp]),
     'f110_vehicle_dynamics_st': (C.c_int, [_dp, _dp, _dp, C.c_int32, _dp, _dp]),
     'f110_vehicle_dynamics_ks': (C.c_int, [_dp, _dp, _dp, C.c_int32, _dp, _dp]),
     'f110_pid': (C.c_int, [_dp, _dp, C.c_int32, _dp, _dp]),
@@ -148,6 +167,7 @@ DEBUG_SIGNATURES = {
     'f110_debug_set_tail': (None, [C.c_int]),
     'f110_debug_set_tail2': (None, [C.c_int, C.c_int]),
     'f110_debug_set_tile_counter': (None, [C.c_void_p]),
+    'f110_debug_set_obst_events': (None, [C.c_void_p, C.c_void_p, C.c_void_p]),
     'f110_debug_last_launch': (C.c_char_p, []),
 }
 

@@ -22,6 +22,12 @@ __device__ __forceinline__ void get_vertices_cs(double px, double py, double c, 
     }
 }
 
+// an obstacle slot (f110_obstacles.boxes row, active byte) takes part only when it is active, its pose is finite and its size finite and > 0
+__device__ __forceinline__ bool box_present(const double *b, uint8_t act) {
+    return act && isfinite(b[0]) && isfinite(b[1]) && isfinite(b[2]) && isfinite(b[3]) && isfinite(b[4]) && b[3] > 0.0 &&
+           b[4] > 0.0;
+}
+
 __device__ __forceinline__ void get_vertices(double px, double py, double th, double length, double width,
                                              double v[8]) {
     double c = cos(th), s = sin(th);

@@ -951,6 +951,10 @@ __global__ void __launch_bounds__(F110_TAIL_NOSCAN_THREADS) k_tail_noscan(f110_s
     }
 }
 
+}  // namespace f110
+#include "obstacles.cuh"     // k_obstacles, k_env_tail_obst: built on the tail's device functions above
+namespace f110 {
+
 // f110_track_progress_sum: the deltas of the ticks of one policy step, summed in tick order
 __global__ void k_delta_sum(const double *__restrict__ delta, double *__restrict__ sum, int n, int restart) {
     const int a = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1838,13 +1842,17 @@ struct TailShape {
     bool separate;                   // FINALIZE standing in for the fused tail (more than 32 agents per env)
 };
 
+// largest value a scan entry can hold: the max_range clamp plus 8 sigma of the optional noise
+static double max_scan_range(const f110_sim *sim, const f110_map *map) {
+    return map->max_range + 8.0 * (sim->noise_std > 0.0 ? sim->noise_std : 0.0) + 1e-3;
+}
+
 static int launch_tail(const f110_sim *sim, const f110_map *map, const BeamView &bv, const TailOpts *tail, bool pdl, cudaStream_t st,
                        TailShape *shape) {
     const int NA = sim->num_envs * sim->num_agents;
     const bool fused = tail && tail->fused;
     TailShape &ts = *shape;
-    // largest value a scan entry can hold: the max_range clamp plus 8 sigma of the optional noise
-    const double max_scan = map->max_range + 8.0 * (sim->noise_std > 0.0 ? sim->noise_std : 0.0) + 1e-3;
+    const double max_scan = max_scan_range(sim, map);
     // k_tail2 (2 <= A <= 4): faster than k_tail at cfg3 and, once its blocks are small enough to fill the GPU, at cfg2x2
     if (sim->num_agents >= 2 && sim->num_agents <= 4 && g_tail2) {
         // two-phase tail: ~64 agents per block (thread per (ego, opponent) pair for the scalar work, warp per ego for the beams);
@@ -1963,14 +1971,70 @@ static void write_launch_record(const MarchPlan &p, const MapGeom &geom, const f
              p.rot && p.lean ? "" : " ROT=0", p.mq.static_runs, p.per_warp, tail);
 }
 
+// ------------------------------------------------------------------------------------ obstacles (csrc/obstacles.cuh)
+struct ObstPlan {
+    ObstK k;
+    ObstDraw d;
+};
+// f110_obstacles -> the kernels' views, every rule of the header checked before anything is enqueued.  num_layers: the map's
+// layer count that per-layer candidate tables must match, or -1 when the call has no map.
+static int plan_obstacles(const f110_sim *sim, const f110_obstacles *o, int num_layers, ObstPlan *p) {
+    if (o->per_env < 1 || o->per_env > F110_MAX_OBSTACLES || !o->boxes || !o->active) return F110_ERR_INVALID;
+    if (o->count_min < 0 || o->count_min > o->count_max || o->count_max > o->per_env) return F110_ERR_INVALID;
+    if (!(o->clearance >= 0.0) || !isfinite(o->clearance)) return F110_ERR_INVALID;
+    p->k.boxes = o->boxes; p->k.active = o->active; p->k.hit = o->hit; p->k.K = o->per_env;
+    ObstDraw &d = p->d;
+    memset(&d, 0, sizeof(d));
+    d.boxes = o->boxes; d.active = o->active; d.cand = o->candidates; d.K = o->per_env;
+    d.num_cand = o->num_candidates; d.num_tables = 0;
+    d.count_min = o->count_min; d.count_max = o->count_max; d.clearance = o->clearance; d.seed = o->seed;
+    if (!o->candidates) return F110_OK;
+    if (o->num_candidates < 1) return F110_ERR_INVALID;
+    if (!o->cand_offsets) return F110_OK;
+    const int L = o->num_cand_tables;
+    if (L < 1 || L > F110_MAX_START_TABLES || !sim->env_layer || o->cand_offsets[0] != 0 || o->cand_offsets[L] != o->num_candidates)
+        return F110_ERR_INVALID;
+    if (num_layers >= 0 && L != std::max(num_layers, 1)) return F110_ERR_INVALID;
+    for (int l = 0; l <= L; l++) {
+        if (l < L && o->cand_offsets[l + 1] <= o->cand_offsets[l]) return F110_ERR_INVALID;
+        d.off[l] = o->cand_offsets[l];
+    }
+    d.num_tables = L;
+    return F110_OK;
+}
+// measurement aid (f110_debug_set_obst_events): events recorded before k_obstacles, after it, and after k_env_tail_obst
+static cudaEvent_t g_obst_ev[3] = {nullptr, nullptr, nullptr};
+// after the tail of a tick that ran without its env-level part: k_obstacles, then (a tick with lap logic or auto-reset)
+// k_env_tail_obst.  tail NULL: f110_step.  rd: the repeat bookkeeping of an intermediate tick of f110_tick_repeat, or NULL.
+static int launch_obst_tail(const f110_sim *sim, const BeamView &bv, const ObstPlan &ob, const TailOpts *tail, bool scan,
+                            const RepeatDone *rd, double max_scan, cudaStream_t st) {
+    const int NA = sim->num_envs * sim->num_agents;
+    const unsigned grid = (unsigned)(((long long)NA * 32 + 127) / 128);
+    if (g_obst_ev[0]) CUDA_TRY(cudaEventRecord(g_obst_ev[0], st));
+    if (scan) k_obstacles<true><<<grid, 128, 0, st>>>(*sim, bv, ob.k, max_scan);
+    else k_obstacles<false><<<grid, 128, 0, st>>>(*sim, bv, ob.k, max_scan);
+    LAUNCH_CHECK("k_obstacles");
+    if (g_obst_ev[1]) CUDA_TRY(cudaEventRecord(g_obst_ev[1], st));
+    if (tail && (tail->env_level || tail->ar.start_poses)) {
+        RepeatDone r;
+        r.done_any = rd ? rd->done_any : nullptr; r.done_tick = rd ? rd->done_tick : nullptr; r.tick = rd ? rd->tick : 0;
+        k_env_tail_obst<<<(sim->num_envs + 127) / 128, 128, 0, st>>>(*sim, (int)tail->env_level, tail->ar, r, ob.d);
+        LAUNCH_CHECK("k_env_tail_obst");
+    }
+    if (g_obst_ev[2]) CUDA_TRY(cudaEventRecord(g_obst_ev[2], st));
+    return F110_OK;
+}
+
 // ------------------------------------------------------------------------------------ the plan and the launches of a tick
 struct TickPlan {
     MapGeom geom;
     MarchPlan march;
+    const ObstPlan *obst;    // NULL: no obstacles (the tail runs as before)
 };
 static int plan_tick(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                      const double *actions, TickPlan *tp) {
     int rc;
+    tp->obst = nullptr;
     if ((rc = check_sim(sim)) || (rc = check_map(map)) || (rc = check_beams(beams))) return rc;
     if (!actions) return F110_ERR_INVALID;
     if (sim->lookup_counter && sim->noise_std > 0.0) return F110_ERR_INVALID;   // counting runs are noise-free by construction
@@ -1992,8 +2056,15 @@ static int launch_tick(const f110_sim *sim, const f110_map *map, const f110_marc
     if ((rc = launch_march_plan(plan, sim, map, tables, beams, tp.geom, pdl, st))) return rc;
     if (ev) CUDA_TRY(cudaEventRecord(ev[2], st));
     TailShape ts = {};
-    if ((rc = launch_tail(sim, map, make_view(beams), tail, pdl && plan.lean, st, &ts))) return rc;
+    const BeamView bv = make_view(beams);
+    // with obstacles the tail runs without its env-level part: contact with a box must be known before `done` and the auto-reset
+    if ((rc = launch_tail(sim, map, bv, tp.obst ? nullptr : tail, pdl && plan.lean, st, &ts))) return rc;
+    if (tp.obst && (rc = launch_obst_tail(sim, bv, *tp.obst, tail, true, nullptr, max_scan_range(sim, map), st))) return rc;
     write_launch_record(plan, tp.geom, map, ts);
+    if (tp.obst) {
+        const size_t n = strlen(g_launch_rec);
+        snprintf(g_launch_rec + n, sizeof(g_launch_rec) - n, " obst=%d", tp.obst->k.K);
+    }
     if (ev) CUDA_TRY(cudaEventRecord(ev[3], st));
     return F110_OK;
 }
@@ -2101,6 +2172,13 @@ static int launch_ttc_tick(const f110_sim *sim, const f110_map *map, const f110_
     const int epb = std::max(1, F110_TAIL_NOSCAN_THREADS / sim->num_agents);
     RepeatDone rd;
     rd.done_any = rep->done_any; rd.done_tick = rep->done_tick; rd.tick = tick;
+    if (rp.tick.obst) {       // the agent part here, then box contact, then the env level with the respawn
+        AutoResetArgs no_ar = tail.ar;
+        no_ar.start_poses = nullptr;
+        k_tail_noscan<<<(sim->num_envs + epb - 1) / epb, F110_TAIL_NOSCAN_THREADS, 0, st>>>(*sim, 0, no_ar, epb, rd);
+        LAUNCH_CHECK("k_tail_noscan");
+        return launch_obst_tail(sim, make_view(beams), *rp.tick.obst, &tail, false, &rd, max_scan_range(sim, map), st);
+    }
     k_tail_noscan<<<(sim->num_envs + epb - 1) / epb, F110_TAIL_NOSCAN_THREADS, 0, st>>>(*sim, (int)tail.env_level, tail.ar, epb, rd);
     LAUNCH_CHECK("k_tail_noscan");
     return F110_OK;
@@ -2146,6 +2224,11 @@ void f110_debug_set_tail(int minb) {      // -1: k_tail always; -2 or a register
     else { g_tail2 = 1; g_tail_minb = minb; }
 }
 void f110_debug_set_tile_counter(unsigned long long *buf) { g_tile_counter = buf; }
+/* measurement aid: three cudaEvent_t (or NULL) recorded around k_obstacles and k_env_tail_obst of every obstacle tick (not
+ * for graph capture: tools/bench_obstacles.py times plain ticks with them) */
+void f110_debug_set_obst_events(void *before, void *between, void *after) {
+    g_obst_ev[0] = (cudaEvent_t)before; g_obst_ev[1] = (cudaEvent_t)between; g_obst_ev[2] = (cudaEvent_t)after;
+}
 void f110_debug_set_chunk(int chunk_shift) { g_chunk = (chunk_shift < 0 || chunk_shift > 6) ? 3 : chunk_shift; }
 /* test aid (not in the public header): `key=value` record of the kernels the last step / tick of the calling thread launched
  * (march kernel family and template choices, queue figures, tail kernel and shape); empty before the first one */
@@ -2169,11 +2252,17 @@ const char *f110_last_cuda_error(void) { return g_cuda_err; }
 // One tick: validate, classify the map, plan the march (all before anything is enqueued: a tick either runs completely or not
 // at all), then k_dynamics, the planned march and the tail, with an event between them when the caller profiles.
 static int step_impl(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
-                     const double *actions, cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail = nullptr) {
+                     const double *actions, cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail = nullptr,
+                     const f110_obstacles *obst = nullptr) {
     int rc;
     g_launch_rec[0] = '\0';
     TickPlan tp;
+    ObstPlan ob;
     if ((rc = plan_tick(sim, map, tables, beams, actions, &tp))) return rc;
+    if (obst) {
+        if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
+        tp.obst = &ob;
+    }
     return launch_tick(sim, map, tables, beams, actions, tp, st, ev, tail);
 }
 
@@ -2183,7 +2272,11 @@ int f110_step(const f110_sim *sim, const f110_map *map, const f110_beams *beams,
 }
 int f110_step_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                  const double *actions, void *stream) {
-    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr);
+    return f110_step_obst(sim, map, tables, beams, actions, nullptr, stream);
+}
+int f110_step_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                   const double *actions, const f110_obstacles *obst, void *stream) {
+    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, nullptr, obst);
 }
 
 int f110_step_profile(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
@@ -2260,6 +2353,10 @@ static int start_tables(const f110_sim *sim, int32_t num_start, AutoResetArgs &a
 
 int f110_autoreset(const f110_sim *sim, const double *start_poses, int32_t num_start, int32_t pose_gap,
                    uint64_t seed, uint64_t tick, void *stream) {
+    return f110_autoreset_obst(sim, start_poses, num_start, pose_gap, seed, tick, nullptr, stream);
+}
+int f110_autoreset_obst(const f110_sim *sim, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
+                        uint64_t tick, const f110_obstacles *obst, void *stream) {
     int rc;
     if ((rc = check_sim(sim))) return rc;
     if (!start_poses || num_start <= 0) return F110_ERR_INVALID;
@@ -2268,8 +2365,28 @@ int f110_autoreset(const f110_sim *sim, const double *start_poses, int32_t num_s
     AutoResetArgs ar;
     ar.start_poses = start_poses; ar.num_start = num_start; ar.pose_gap = pose_gap; ar.seed = seed; ar.tick_host = tick;
     if ((rc = start_tables(sim, num_start, ar))) return rc;
+    if (obst) {
+        ObstPlan ob;
+        if ((rc = plan_obstacles(sim, obst, -1, &ob))) return rc;
+        RepeatDone rd;
+        rd.done_any = nullptr; rd.done_tick = nullptr; rd.tick = 0;
+        k_env_tail_obst<<<(sim->num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*sim, 0, ar, rd, ob.d);
+        LAUNCH_CHECK("k_env_tail_obst");
+        return F110_OK;
+    }
     k_autoreset<<<(sim->num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*sim, ar);
     LAUNCH_CHECK("k_autoreset");
+    return F110_OK;
+}
+
+int f110_obstacles_respawn(const f110_sim *sim, const f110_obstacles *obst, const uint8_t *env_mask, uint64_t tick, void *stream) {
+    int rc;
+    if ((rc = check_sim(sim))) return rc;
+    if (!obst || !obst->candidates || sim->num_agents > 32) return F110_ERR_INVALID;
+    ObstPlan ob;
+    if ((rc = plan_obstacles(sim, obst, -1, &ob))) return rc;
+    k_obst_respawn<<<(sim->num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*sim, ob.d, env_mask, tick);
+    LAUNCH_CHECK("k_obst_respawn");
     return F110_OK;
 }
 
@@ -2297,19 +2414,32 @@ static int tick_tail_opts(const f110_sim *sim, const f110_map *map, int32_t env_
 int f110_tick_ex(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                  const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
                  uint64_t seed, void *stream) {
+    return f110_tick_obst(sim, map, tables, beams, actions, env_level, start_poses, num_start, pose_gap, seed, nullptr, stream);
+}
+int f110_tick_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                   const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                   uint64_t seed, const f110_obstacles *obst, void *stream) {
     int rc;
     TailOpts t;
     if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
-    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, &t);
+    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, &t, obst);
 }
 
 int f110_tick_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                            const double *actions, int32_t repeat, int32_t first_tick, int32_t num_ticks, const f110_repeat *rep,
                            int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
                            void *stream) {
+    return f110_tick_repeat_ticks_obst(sim, map, tables, beams, actions, repeat, first_tick, num_ticks, rep, env_level, start_poses,
+                                       num_start, pose_gap, seed, nullptr, stream);
+}
+int f110_tick_repeat_ticks_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                                const double *actions, int32_t repeat, int32_t first_tick, int32_t num_ticks, const f110_repeat *rep,
+                                int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
+                                const f110_obstacles *obst, void *stream) {
     int rc;
     TailOpts t;
     RepeatPlan rp;
+    ObstPlan ob;
     cudaStream_t st = (cudaStream_t)stream;
     if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
     if (repeat < 1 || repeat > F110_MAX_REPEAT || first_tick < 0 || num_ticks < 1 || first_tick > repeat - num_ticks) return F110_ERR_INVALID;
@@ -2317,6 +2447,10 @@ int f110_tick_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_
     if ((rep->done_any || rep->done_tick) && !env_level) return F110_ERR_INVALID;     // done is computed by the env-level part
     g_launch_rec[0] = '\0';
     if ((rc = plan_repeat(sim, map, tables, beams, actions, repeat, &rp))) return rc;
+    if (obst) {
+        if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
+        rp.tick.obst = &ob;
+    }
 
     if (first_tick == 0) CUDA_TRY(cudaMemsetAsync(rep->list_count, 0, sizeof(uint32_t) * (size_t)repeat, st));
     const bool track_done = rep->done_any || rep->done_tick;
@@ -2541,6 +2675,12 @@ int f110_scan_layers(const f110_map *map, const f110_beams *beams, const double 
 int f110_render_views(const f110_sim *sim, const f110_map *map, const int32_t *agent_ids, int32_t V, int32_t height,
                       int32_t width, double metres_per_pixel, double forward_offset, int32_t heading_up, uint8_t *out,
                       void *stream) {
+    return f110_render_views_obst(sim, map, nullptr, agent_ids, V, height, width, metres_per_pixel, forward_offset, heading_up, out,
+                                  stream);
+}
+int f110_render_views_obst(const f110_sim *sim, const f110_map *map, const f110_obstacles *obst, const int32_t *agent_ids, int32_t V,
+                           int32_t height, int32_t width, double metres_per_pixel, double forward_offset, int32_t heading_up,
+                           uint8_t *out, void *stream) {
     if (!sim || !map || !agent_ids || !out || !sim->state) return F110_ERR_INVALID;
     if (V < 1 || height < 1 || height > F110_RENDER_MAX_SIZE || width < 1 || width > F110_RENDER_MAX_SIZE) return F110_ERR_INVALID;
     if (!isfinite(metres_per_pixel) || !(metres_per_pixel > 0.0) || !isfinite(forward_offset)) return F110_ERR_INVALID;
@@ -2577,6 +2717,11 @@ int f110_render_views(const f110_sim *sim, const f110_map *map, const int32_t *a
     p.num_layers = layers;
     p.NA = sim->num_envs * sim->num_agents; p.A = sim->num_agents;
     p.V = V; p.H = height; p.W = width; p.heading_up = heading_up ? 1 : 0;
+    if (obst) {
+        ObstPlan ob;
+        if ((rc = plan_obstacles(sim, obst, -1, &ob))) return rc;
+        p.boxes = obst->boxes; p.active = obst->active; p.K = obst->per_env;
+    }
     const unsigned long long tiles = ((unsigned long long)height * (unsigned long long)width + F110_RENDER_PIXELS - 1) /
                                      F110_RENDER_PIXELS;
     const dim3 grid((unsigned)tiles, (unsigned)(V < 65535 ? V : 65535)), block(F110_RENDER_THREADS);

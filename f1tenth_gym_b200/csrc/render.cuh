@@ -2,8 +2,9 @@
 //
 // A view of H x W pixels, row 0 at the top, s metres per pixel, follows agent a (flat index).  Every pixel gets one class code:
 //   0 off-map, 1 free (dt != 0), 2 wall (dt == 0, what the lidar sees), 3 another agent of the env, 4 the followed agent,
+//   5 a static box obstacle of the env (f110_obstacles, csrc/obstacles.cuh),
 //   255 the whole view is invalid (agent id outside [0, N*A), env layer outside [0, L), or the followed pose not finite: no table
-//   is read).  Priority 4 > 3 > 2 > 1 / 0.
+//   is read).  Priority 4 > 3 > 5 > 2 > 1 / 0.
 //
 // Operation order (fp64, no FMA contraction: the library is built with -fmad=false; tests/test_views_host.py restates it):
 //   x, y, yaw = state[0][a], state[1][a], state[4][a];   sincos(yaw) -> (sn, cs)   (as k_dynamics)
@@ -23,6 +24,8 @@
 //     (collision.cuh, the routine of k_vertices), vertices rl, rr, fr, fl (counter-clockwise).  Pixel centre p is inside when
 //     bx0 <= px <= bx1 && by0 <= py <= by1 (the vertices' bounding box) and, for each edge (v0 -> v1) in that vertex order,
 //     (v1x - v0x) * (py - v0y) - (v1y - v0y) * (px - v0x) >= 0.
+//   boxes: every present slot k of the env (box_present) is the quad get_vertices_cs(x, y, cos, sin, length, width) with
+//     (sin, cos) = sincos(yaw) (the vertices k_obstacles uses), with the same inside test.
 //
 // A block covers a tile of F110_RENDER_PIXELS consecutive pixels (row-major) of one view and loads the view's pose, its layer's
 // geometry and the env's car quads into shared memory once per view; the grid's y dimension strides over the views.  Every
@@ -35,6 +38,7 @@ namespace f110 {
 #define F110_RENDER_THREADS 256
 #define F110_RENDER_PIXELS (4 * F110_RENDER_THREADS)
 #define F110_RENDER_MAX_AGENTS 64      // car quads cached per block (agents per env)
+#define F110_RENDER_MAX_BOXES 16       // box quads cached per block (f110_obstacles slots per env, F110_MAX_OBSTACLES)
 #define F110_RENDER_MAX_SIZE 8192      // largest view height / width
 
 struct RenderK {
@@ -46,6 +50,8 @@ struct RenderK {
     const double *__restrict__ layer_res;   // [L][2] or NULL
     const double *__restrict__ layer_rot;   // [L][2] or NULL
     uint8_t *__restrict__ out;              // [V][H][W]
+    const double *__restrict__ boxes;       // [N][K][5] obstacle boxes, or NULL (K = 0)
+    const uint8_t *__restrict__ active;     // [N][K]
     double2 orig, ext, rot;                 // struct geometry: (orig_x, orig_y), (W res, H res), (orig_c, orig_s)
     double res;
     double length, width;                   // sim_length, sim_width
@@ -54,6 +60,7 @@ struct RenderK {
     unsigned map_w, map_h;                  // canvas (or map) width / height
     unsigned num_layers;                    // >= 1
     int NA, A, V, H, W, heading_up;
+    int K;                                  // obstacle slots per env, 0 = none
 };
 
 struct RenderView {
@@ -66,8 +73,9 @@ struct RenderView {
 
 __global__ void __launch_bounds__(F110_RENDER_THREADS) k_render_views(const RenderK p) {
     __shared__ RenderView sv;
-    __shared__ double4 s_box[F110_RENDER_MAX_AGENTS];          // bounding box (x0, x1, y0, y1); empty for a car not drawn
-    __shared__ double s_vert[F110_RENDER_MAX_AGENTS][8];
+    // entries 0 .. A-1: the env's cars; A .. A+K-1: its obstacle boxes
+    __shared__ double4 s_box[F110_RENDER_MAX_AGENTS + F110_RENDER_MAX_BOXES];   // bounding box (x0, x1, y0, y1); empty: not drawn
+    __shared__ double s_vert[F110_RENDER_MAX_AGENTS + F110_RENDER_MAX_BOXES][8];
     const unsigned long long HW = (unsigned long long)p.H * (unsigned long long)p.W;
     const unsigned long long lin0 = (unsigned long long)blockIdx.x * F110_RENDER_PIXELS + 4ull * threadIdx.x;
     for (long long vi = blockIdx.y; vi < p.V; vi += gridDim.y) {       // 64-bit: no overflow for V near INT32_MAX
@@ -125,6 +133,23 @@ __global__ void __launch_bounds__(F110_RENDER_THREADS) k_render_views(const Rend
             s_box[threadIdx.x] = b;
 #pragma unroll
             for (int q = 0; q < 8; q++) s_vert[threadIdx.x][q] = v[q];
+        } else if (sv.valid && threadIdx.x < (unsigned)(p.A + p.K)) {
+            const int env = __ldg(p.agent_ids + vi) / p.A, k = (int)threadIdx.x - p.A;
+            const double *bx = p.boxes + ((size_t)env * p.K + k) * 5;
+            double v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            double4 b = make_double4(INFINITY, -INFINITY, INFINITY, -INFINITY);
+            if (box_present(bx, p.active[(size_t)env * p.K + k])) {
+                double sn, cs;
+                sincos(bx[2], &sn, &cs);
+                get_vertices_cs(bx[0], bx[1], cs, sn, bx[3], bx[4], v);
+                b.x = fmin(fmin(v[0], v[2]), fmin(v[4], v[6]));
+                b.y = fmax(fmax(v[0], v[2]), fmax(v[4], v[6]));
+                b.z = fmin(fmin(v[1], v[3]), fmin(v[5], v[7]));
+                b.w = fmax(fmax(v[1], v[3]), fmax(v[5], v[7]));
+            }
+            s_box[threadIdx.x] = b;
+#pragma unroll
+            for (int q = 0; q < 8; q++) s_vert[threadIdx.x][q] = v[q];
         }
         __syncthreads();
         if (lin0 >= HW) continue;
@@ -161,6 +186,19 @@ __global__ void __launch_bounds__(F110_RENDER_THREADS) k_render_views(const Rend
                         if (k == sv.self) { c = 4; break; }
                         c = 3;
                     }
+                }
+                for (int k = p.A; c == 0 && k < p.A + p.K; k++) {
+                    const double4 b = s_box[k];
+                    if (!(px >= b.x && px <= b.y && py >= b.z && py <= b.w)) continue;
+                    const double *vk = s_vert[k];
+                    bool in = true;
+#pragma unroll
+                    for (int e = 0; e < 4; e++) {
+                        const int e2 = (e + 1) & 3;
+                        const double ex = vk[2 * e2] - vk[2 * e], ey = vk[2 * e2 + 1] - vk[2 * e + 1];
+                        in = in && (ex * (py - vk[2 * e + 1]) - ey * (px - vk[2 * e]) >= 0.0);
+                    }
+                    if (in) c = 5;
                 }
                 if (c == 0) {
                     const double tx = px - sv.ox, ty = py - sv.oy;

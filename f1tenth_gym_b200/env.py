@@ -27,6 +27,10 @@ one simulator (DeviceMap.stack: one resolution, unrotated origins); env e drives
 mixed_resolution=True also stacks maps of different resolutions (e.g. generated tracks with the bundled maps); every map
 of such a batch is then marched in metres, the power-of-two ones included.  rotated_origins=True also stacks maps whose
 yaml origin has a yaw (marched in metres in each map's rotated frame by k_march_lean_rot).
+obstacles={'candidates': (C, 5) table or one per map, 'count': (lo, hi), 'clearance': m, 'seed': s} (batched mode only;
+Simulator.set_obstacles / set_obstacle_draw with hi slots per env): static box obstacles, redrawn on the device for every env by
+reset() after it places the agents and for the masked envs by reset_envs(); obs['obstacles'] (N, K, 5) and
+obs['obstacle_active'] (N, K) are views of the device buffers, and local_map / rgb_array draw the boxes (class 5).
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
@@ -69,6 +73,7 @@ class F110Env(object):
         self.num_envs = int(num_envs) if self.batched else 1
         if isinstance(self.map_path, (list, tuple)) and not self.batched:
             raise ValueError('a list of maps needs the batched mode (num_envs)')
+        self._obstacles = self._obstacle_settings(kwargs.get('obstacles', None), self.batched)
         self.start_thresh = 0.5
         self.sim = Simulator(self.params, self.num_agents, self.seed, time_step=self.timestep,
                              ego_idx=self.ego_idx, integrator=self.integrator, lidar_dist=self.lidar_dist,
@@ -89,6 +94,10 @@ class F110Env(object):
             raise ValueError('action_repeat must be an int in [1, 64], got %r' % (self.action_repeat,))
         self.action_repeat = int(self.action_repeat)
         self._set_map(self.map_path, self.map_ext)
+        if self._obstacles is not None:
+            cand, count, clearance, seed = self._obstacles
+            self.sim.set_obstacles(np.zeros((count[1], 5)), np.zeros(count[1], bool))
+            self.sim.set_obstacle_draw(cand, count=count, clearance=clearance, seed=seed)
         self.render_obs = None
         self._local_map_buf = None
         self._palette = None
@@ -131,6 +140,7 @@ class F110Env(object):
                 obs['local_map'] = self._render_local_map()
             obs['lap_times'] = sim.lap_times.view(N, A)
             obs['lap_counts'] = sim.lap_counts.view(N, A)
+            self._obstacle_obs(obs)
             if self.centerline is not None:
                 p = sim.update_progress()
                 for k, v in PROGRESS_KEYS:
@@ -201,6 +211,7 @@ class F110Env(object):
         a = action if torch.is_tensor(action) else np.asarray(action, dtype=np.float64).reshape(N, A, 2)
         obs = sim.tick_repeat(a, K, env_level=True, progress=tracked)
         obs['lap_times'], obs['lap_counts'] = sim.lap_times.view(N, A), sim.lap_counts.view(N, A)
+        self._obstacle_obs(obs)
         if self._local_map is not None:
             obs['local_map'] = self._render_local_map()
         reward = K * self.timestep
@@ -226,14 +237,44 @@ class F110Env(object):
         """f110_env.py:306-349: zero counters, start frame, Simulator.reset, then ONE zero-action tick
         whose (obs, reward, done, info) is returned."""
         self.sim.env_reset(poses)
+        if self._obstacles is not None:
+            self.sim.respawn_obstacles()
         action = torch.zeros((self.num_envs, self.num_agents, 2), dtype=torch.float64, device=self.sim.device)
         if not self.batched:
             return self._step_single(action)
         return self._finish(self.sim.step(action))
 
     def reset_envs(self, env_mask, poses):
-        """Batch extension: re-initialise only the masked envs (counters + Simulator.reset); no tick is run."""
+        """Batch extension: re-initialise only the masked envs (counters + Simulator.reset, then their obstacles are redrawn);
+        no tick is run."""
         self.sim.env_reset(poses, env_mask)
+        if self._obstacles is not None:
+            self.sim.respawn_obstacles(env_mask)
+
+    def _obstacle_obs(self, obs):
+        if self._obstacles is not None:
+            obs['obstacles'], obs['obstacle_active'] = self.sim.obstacle_boxes, self.sim.obstacle_active
+
+    @staticmethod
+    def _obstacle_settings(cfg, batched):
+        """obstacles kwarg -> (candidates, (lo, hi), clearance, seed), or None; ValueError before any device work."""
+        if cfg is None:
+            return None
+        if not batched:
+            raise ValueError('obstacles need the batched mode (num_envs)')
+        if not isinstance(cfg, dict) or 'candidates' not in cfg or set(cfg) - {'candidates', 'count', 'clearance', 'seed'}:
+            raise ValueError("obstacles must be a dict with 'candidates' and optionally 'count', 'clearance', 'seed', got %r"
+                             % (cfg,))
+        try:
+            lo, hi = (int(v) for v in cfg.get('count', (1, 1)))
+        except (TypeError, ValueError):
+            raise ValueError('obstacles count must be (lo, hi), got %r' % (cfg.get('count'),))
+        if not 0 <= lo <= hi or not 1 <= hi <= 16:
+            raise ValueError('obstacles count must satisfy 0 <= lo <= hi, 1 <= hi <= 16, got %r' % (cfg.get('count'),))
+        clearance = float(cfg.get('clearance', 1.0))
+        if not (np.isfinite(clearance) and clearance >= 0.0):
+            raise ValueError('obstacles clearance must be finite and >= 0, got %r' % clearance)
+        return cfg['candidates'], (lo, hi), clearance, int(cfg.get('seed', 0))
 
     def update_map(self, map_path, map_ext, env_map_ids=None, mixed_resolution=None, rotated_origins=None, centerline=None):
         """f110_env.py:351-362.  Batch extension: lists of map paths (and extensions) as in the constructor;
@@ -343,3 +384,4 @@ RENDER_PALETTE[0] = RENDER_PALETTE[1] = (9, 32, 87)
 RENDER_PALETTE[2] = (183, 193, 222)
 RENDER_PALETTE[3] = (99, 52, 94)
 RENDER_PALETTE[4] = (172, 97, 185)
+RENDER_PALETTE[5] = (236, 146, 38)      # static obstacles

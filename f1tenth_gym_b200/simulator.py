@@ -410,6 +410,10 @@ class Simulator(object):
         self._repeat_c = None
         self._repeat_ticks = 0      # intermediate agent-ticks issued since the counter was last read (marched_fraction)
         self._repeat_plain = False
+        # static box obstacles (C ABI f110_obstacles), set by set_obstacles
+        self._obst = None
+        self.obstacle_boxes = self.obstacle_active = self.obstacle_hit = None
+        self._obst_keep = ()
 
     # ------------------------------------------------------------------ configuration
     def set_map(self, map_path, map_ext, edt='scipy'):
@@ -541,8 +545,8 @@ class Simulator(object):
     def step(self, control_inputs):
         """Simulator.step (base_classes.py:553-612). control_inputs (N,A,2) = (steer, speed)."""
         a = self._actions_tensor(control_inputs)
-        nat.check(nat.lib().f110_step_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                         C.byref(self.beams.c), nat.ptr(a), _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_step_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                           C.byref(self.beams.c), nat.ptr(a), self._obst_ref(), _stream_ptr(self.device)))
         return self.observations()
 
     def env_post_step(self):
@@ -574,18 +578,114 @@ class Simulator(object):
         """Reset every env whose ego collided to a hashed draw from start_poses (device (K,3) fp64, or a list of one
         (K_l,3) table per layer of a stacked map)."""
         table, n = self._start_table(start_poses)
-        nat.check(nat.lib().f110_autoreset(C.byref(self.c), nat.ptr(table), n, pose_gap, int(seed), 0,
-                                           _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_autoreset_obst(C.byref(self.c), nat.ptr(table), n, pose_gap, int(seed), 0, self._obst_ref(),
+                                                _stream_ptr(self.device)))
 
     def tick(self, control_inputs, env_level=True, autoreset_poses=None, pose_gap=23, seed=12345):
         """One whole tick in three launches (C ABI f110_tick): step + lap logic + optional auto-reset, same
         results as step(); env_post_step(); autoreset()."""
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
-        nat.check(nat.lib().f110_tick_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                         C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
-                                         int(seed), _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_tick_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                           C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
+                                           int(seed), self._obst_ref(), _stream_ptr(self.device)))
         return self.observations()
+
+    # ------------------------------------------------------------------ static box obstacles
+    def _obst_ref(self):
+        return None if self._obst is None else C.byref(self._obst)
+
+    def _no_obstacles(self, who):
+        if self._obst is not None:
+            raise ValueError('%s does not simulate obstacles; call clear_obstacles() first or use step / tick' % who)
+
+    def set_obstacles(self, boxes, active=None):
+        """Static box obstacles (C ABI f110_obstacles, csrc/obstacles.cuh): parked cars of an env without a sensor that never
+        move.  Every agent's scan is clipped against the boxes of its env, contact sets collisions (collision_idx = A + slot)
+        without zeroing state, and the iTTC check does not see them.  boxes: (K, 5) rows (x, y, yaw, length, width) for every
+        env, or (N, K, 5); 1 <= K <= 16.  active: (K,) or (N, K) bools, default all.  A slot that is inactive, not finite or of
+        size <= 0 is absent.  The data land in obstacle_boxes (N, K, 5) / obstacle_active (N, K), which every tick reads afresh
+        (write into them to move boxes, also under a captured graph); obstacle_hit (N*A,) int32 gets the highest slot each
+        agent touched on the last tick, -1 = none.  Keeps the respawn draw of set_obstacle_draw when K is unchanged."""
+        N = self.num_envs
+        b = torch.as_tensor(boxes, dtype=torch.float64)
+        if b.dim() == 2:
+            b = b.unsqueeze(0).expand(N, -1, -1)
+        if b.dim() != 3 or b.shape[0] != N or b.shape[2] != 5 or not 1 <= b.shape[1] <= nat.MAX_OBSTACLES:
+            raise ValueError('boxes must be (K, 5) or (num_envs, K, 5) with 1 <= K <= %d, got %s'
+                             % (nat.MAX_OBSTACLES, tuple(b.shape)))
+        K = b.shape[1]
+        act = torch.ones((N, K), dtype=torch.bool) if active is None else torch.as_tensor(active).to(torch.bool)
+        if act.dim() == 1:
+            act = act.unsqueeze(0).expand(N, -1)
+        if tuple(act.shape) != (N, K):
+            raise ValueError('active must be (K,) or (num_envs, K) with K = %d, got %s' % (K, tuple(act.shape)))
+        if self._obst is None or self._obst.per_env != K:
+            dev = self.device
+            self.obstacle_boxes = torch.zeros((N, K, 5), dtype=torch.float64, device=dev)
+            self.obstacle_active = torch.zeros((N, K), dtype=torch.uint8, device=dev)
+            self.obstacle_hit = torch.full((N * self.num_agents,), -1, dtype=torch.int32, device=dev)
+            self._obst = nat.F110Obstacles(K, nat.ptr(self.obstacle_boxes), nat.ptr(self.obstacle_active),
+                                           nat.ptr(self.obstacle_hit), None, None, 0, 0, 0, 0, 0.0, 0)
+            self._obst_keep = ()
+            self._graph = None
+        self.obstacle_boxes.copy_(b)
+        self.obstacle_active.copy_(act.to(torch.uint8))
+
+    def set_obstacle_draw(self, candidates, count=(1, 1), clearance=1.0, seed=0):
+        """Redraw an env's boxes whenever the auto-reset restarts it (and on respawn_obstacles): candidates is one (C, 5) table of
+        boxes for every env, or for a stacked map a list of one table per layer; slot k takes a hashed row of its env's table,
+        count = (lo, hi) slots are active (uniform, lo <= hi <= K), and a box whose centre lies closer than `clearance` metres to
+        an agent's new position stays inactive.  The draw is f1tenth_gym_b200.obstacles.respawn_draw.  Needs set_obstacles."""
+        if self._obst is None:
+            raise ValueError('set_obstacle_draw needs set_obstacles first')
+        K = self._obst.per_env
+        try:
+            lo, hi = (int(v) for v in count)
+        except (TypeError, ValueError):
+            raise ValueError('count must be (lo, hi), got %r' % (count,))
+        if not 0 <= lo <= hi <= K:
+            raise ValueError('count must satisfy 0 <= lo <= hi <= K = %d, got %r' % (K, count))
+        clearance = float(clearance)
+        if not (np.isfinite(clearance) and clearance >= 0.0):
+            raise ValueError('clearance must be finite and >= 0, got %r' % clearance)
+        per_layer = isinstance(candidates, (list, tuple))
+        tabs = list(candidates) if per_layer else [candidates]
+        tabs = [torch.as_tensor(np.asarray(t) if not torch.is_tensor(t) else t, dtype=torch.float64).reshape(-1, 5) for t in tabs]
+        if any(t.shape[0] < 1 or not bool(torch.isfinite(t).all()) for t in tabs):
+            raise ValueError('every candidate table needs at least one finite (x, y, yaw, length, width) row')
+        layers = getattr(self._map_struct, 'num_layers', 1)
+        offs = None
+        if per_layer:
+            if layers <= 1 or self.env_layer is None or len(tabs) != layers:
+                raise ValueError('candidates as a list needs one table per layer of the stacked map (%d)' % max(layers, 1))
+            offs = np.concatenate([[0], np.cumsum([t.shape[0] for t in tabs])]).astype(np.int32)
+        cand = torch.cat(tabs).to(self.device).contiguous()
+        self._obst_offsets = None if offs is None else (C.c_int32 * offs.size)(*offs.tolist())
+        self._obst_keep = (cand,)
+        o = self._obst
+        o.candidates, o.num_candidates = nat.ptr(cand), cand.shape[0]
+        o.cand_offsets = None if offs is None else C.addressof(self._obst_offsets)
+        o.num_cand_tables = 0 if offs is None else layers
+        o.count_min, o.count_max, o.clearance = lo, hi, clearance
+        o.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self._graph = None
+
+    def respawn_obstacles(self, env_mask=None):
+        """The respawn draw for the masked envs (None: all) around the agents' current positions, at the current tick counter
+        (reads it: one host synchronisation).  Call it after placing the agents."""
+        if self._obst is None or not self._obst.candidates:
+            raise ValueError('respawn_obstacles needs set_obstacles and set_obstacle_draw first')
+        m, mp = self._mask_ptr(env_mask)
+        nat.check(nat.lib().f110_obstacles_respawn(C.byref(self.c), C.byref(self._obst), mp, int(self.tick_counter.item()),
+                                                   _stream_ptr(self.device)))
+
+    def clear_obstacles(self):
+        """Remove every obstacle: the simulator runs exactly as without them."""
+        self._obst = None
+        self.obstacle_boxes = self.obstacle_active = self.obstacle_hit = None
+        self._obst_keep = ()
+        self._graph = None
 
     def _repeat_struct(self):
         """The f110_repeat outputs and scratch, allocated once."""
@@ -609,10 +709,10 @@ class Simulator(object):
         """Enqueue one f110_tick_repeat call; progress: the tracker is updated after every tick of the call (the same ticks,
         issued one by one) and track_delta_sum gets the sum of the call's deltas."""
         def ticks(first, count):
-            nat.check(L.f110_tick_repeat_ticks(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                               C.byref(self.beams.c), nat.ptr(actions), K, first, count, C.byref(call),
-                                               1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(seed),
-                                               _stream_ptr(self.device)))
+            nat.check(L.f110_tick_repeat_ticks_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                                    C.byref(self.beams.c), nat.ptr(actions), K, first, count, C.byref(call),
+                                                    1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(seed),
+                                                    self._obst_ref(), _stream_ptr(self.device)))
         if not progress:
             ticks(0, K)
             return
@@ -757,7 +857,8 @@ class Simulator(object):
     def render_views(self, agent_ids=None, size=(64, 64), metres_per_pixel=0.1, forward_offset=0.0, heading_up=True,
                      out=None):
         """Top-down class views (C ABI f110_render_views, csrc/render.cuh) -> uint8 (V, H, W) on the device: 0 off-map,
-        1 free, 2 wall (dt == 0), 3 another agent of the env, 4 the followed agent, 255 an invalid view.  View k follows flat
+        1 free, 2 wall (dt == 0), 3 another agent of the env, 4 the followed agent, 5 a static obstacle (set_obstacles), 255 an
+        invalid view.  View k follows flat
         agent agent_ids[k] (None: every agent, (N*A, H, W), which reshapes to (N, A, H, W)), centred forward_offset metres
         ahead of it, with its heading up or world-aligned; size = (H, W) pixels of metres_per_pixel each.
         Ids given on the host (int, sequence, numpy, CPU tensor) are range-checked (ValueError); a CUDA tensor must be int32
@@ -779,8 +880,8 @@ class Simulator(object):
                   and tuple(out.shape) == (V, H, W)):
             # (self.state.device, not self.device: device='cuda' has no index, the tensors allocated on it have one)
             raise ValueError('out must be a contiguous uint8 tensor of shape %s on %s' % ((V, H, W), self.state.device))
-        nat.check(nat.lib().f110_render_views(C.byref(self.c), C.byref(self._map_struct), nat.ptr(ids), V, H, W, s, f,
-                                              1 if heading_up else 0, nat.ptr(out), _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_render_views_obst(C.byref(self.c), C.byref(self._map_struct), self._obst_ref(), nat.ptr(ids), V,
+                                                   H, W, s, f, 1 if heading_up else 0, nat.ptr(out), _stream_ptr(self.device)))
         return out
 
     @staticmethod
@@ -839,7 +940,7 @@ class Simulator(object):
                  'start_ys', 'start_thetas', 'start_rot', 'done', 'checkpoint_done', 'tick_counter', 'march_cost',
                  'march_order', 'march_count', 'march_rec', 'track_seg', 'track_s', 'track_d', 'track_heading_error',
                  'track_progress', 'track_delta', 'done_any', 'done_tick', 'repeat_list', 'repeat_list_count',
-                 'marched_agents', 'track_delta_sum')
+                 'marched_agents', 'track_delta_sum', 'obstacle_boxes', 'obstacle_active', 'obstacle_hit')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
 
@@ -847,9 +948,9 @@ class Simulator(object):
             if K > 1:
                 self._issue_repeat(L, actions, K, call, env_level, table, num_start, pose_gap, autoreset_seed, progress)
                 return
-            nat.check(L.f110_tick_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                     C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
-                                     pose_gap, int(autoreset_seed), _stream_ptr(self.device)))
+            nat.check(L.f110_tick_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                       C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
+                                       pose_gap, int(autoreset_seed), self._obst_ref(), _stream_ptr(self.device)))
             if progress:
                 self._launch_progress(L)
         side = torch.cuda.Stream(self.device)
@@ -866,7 +967,8 @@ class Simulator(object):
             tick()
         self._graph = g
         self._graph_keep = (actions, table) + ((self.centerlines, self._progress_views) if progress else ()) + \
-            ((call,) if K > 1 else ())
+            ((call,) if K > 1 else ()) + ((self._obst, self.obstacle_boxes, self.obstacle_active, self.obstacle_hit) +
+                                          self._obst_keep if self._obst is not None else ())
         return g
 
     def replay(self):
@@ -900,7 +1002,8 @@ class Simulator(object):
 
     def step_host(self, io):
         """One tick through HOST buffers (C ABI f110_step_host): H2D actions, step, env_post_step,
-        D2H observation, stream sync.  io from make_host_io(); fill io['actions'] first."""
+        D2H observation, stream sync.  io from make_host_io(); fill io['actions'] first.  ValueError with obstacles set."""
+        self._no_obstacles('step_host')
         nat.check(nat.lib().f110_step_host(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c),
                                            nat.ptr(io['actions']), nat.ptr(self._actions_dev),
                                            C.byref(io['_struct']), _stream_ptr(self.device)))
@@ -956,7 +1059,9 @@ class Simulator(object):
     def step_host_async(self, io):
         """Enqueue one tick whose observation lands in io's pinned host buffers (C ABI f110_step_host_async);
         returns immediately.  Call wait_host(io) before reading them or before reusing io.  With a packed io, ValueError
-        (before anything is enqueued) when the map or the noise changed since the last check and now reaches 32 m."""
+        (before anything is enqueued) when the map or the noise changed since the last check and now reaches 32 m.  ValueError
+        with obstacles set."""
+        self._no_obstacles('step_host_async')
         if io['scans_u24'] is not None:
             checked = io.get('_packed_checked')
             if checked is None or checked[0] is not self._map_struct or checked[1] != self.c.noise_std:
@@ -974,7 +1079,9 @@ class Simulator(object):
         io['_ev_copy'].synchronize()
 
     def step_profile(self, control_inputs):
-        """One tick with CUDA events around each kernel -> (dynamics_ms, raymarch_ms, finalize_ms)."""
+        """One tick with CUDA events around each kernel -> (dynamics_ms, raymarch_ms, finalize_ms).  ValueError with obstacles
+        set."""
+        self._no_obstacles('step_profile')
         a = self._actions_tensor(control_inputs)
         ms = (C.c_float * 3)()
         nat.check(nat.lib().f110_step_profile_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),

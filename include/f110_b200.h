@@ -279,6 +279,73 @@ int f110_tick_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_
                            int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
                            void *stream);
 
+/* ---- static box obstacles (batch extension; csrc/obstacles.cuh) ---- */
+/* An obstacle is a parked car of its env that has no sensor and never moves: an oriented box in env e, slot k.  With boxes of
+ * the size of the agents' bodies (sim_length x sim_width, and the params length / width the opponent ray-cast uses), an env
+ * with K boxes gives its A agents exactly what the reference gives agents 0..A-1 of a Simulator with A + K agents whose agents
+ * A..A+K-1 start at the boxes' poses and receive the action (0, 0) every tick (pid then gives accl = sv = 0, and the RK4 step of
+ * a resting car is the identity):
+ *   - lidar: every agent's scan is clipped against every present box of its env by ray_cast_agents (laser_models.py:206-227,
+ *     :282-346): the blocked-view window, get_range, min(scan, fp32(range)), from the same pose snapshot and with the yaw an
+ *     iTTC hit zeroed (base_classes.py:246-249); scan noise is not applied to the box returns, as to opponent returns;
+ *   - contact: GJK (collision_models.py:113-212) of the agent's body against the box sets collisions[a] = 1 and
+ *     collision_idx[a] = max(.., A + k), the index a parked agent in slot A + k would get.  Contact zeroes no state (neither does
+ *     opponent contact); an ego contact sets done and triggers the auto-reset like any other collision;
+ *   - iTTC: boxes are invisible to it, as opponents are in the reference (check_ttc runs on the wall-only scan).
+ * A slot that is inactive, or whose pose is not finite or whose length or width is not finite and > 0, is absent; with no slot
+ * present every output equals the call without obstacles bit for bit.  The buffers are read afresh by every tick: a caller may
+ * move boxes between ticks, also under a captured CUDA graph. */
+#define F110_MAX_OBSTACLES 16
+typedef struct {
+    int32_t per_env;                /* K, 1 <= K <= F110_MAX_OBSTACLES */
+    double *boxes;                  /* [N][K][5] (x, y, yaw, length, width), device */
+    uint8_t *active;                /* [N][K] device, 0 = absent */
+    int32_t *hit;                   /* [N*A] i32 device, or NULL: the highest slot the agent's body touches this tick, -1 = none */
+    /* the respawn draw: when the auto-reset restarts an env, its boxes are redrawn from these candidates (NULL: boxes stay) */
+    const double *candidates;       /* [C][5] device, rows of the layout of boxes */
+    const int32_t *cand_offsets;    /* [num_cand_tables + 1] HOST memory (read at enqueue, as f110_sim.start_offsets), or NULL:
+                                       an env on layer l draws from rows [cand_offsets[l], cand_offsets[l+1]); needs env_layer,
+                                       offsets from 0 to C rising strictly, num_cand_tables == the map's num_layers
+                                       (checked by the calls that take the map; f110_autoreset_obst and
+                                       f110_obstacles_respawn have none: there an env whose layer has no table gets
+                                       every slot inactive) */
+    int32_t num_candidates;         /* C >= 1 */
+    int32_t num_cand_tables;
+    int32_t count_min, count_max;   /* the active count of a respawn, uniform in [count_min, count_max], 0 <= min <= max <= K */
+    double clearance;               /* a drawn box whose centre is closer than this to an agent's new position stays inactive */
+    uint64_t seed;
+} f110_obstacles;
+
+/* The entry points below take `obst`; NULL is exactly the call without _obst (f110_step_ex, f110_tick_ex,
+ * f110_tick_repeat_ticks, f110_autoreset), which are these with NULL.  With obstacles the tail of a tick runs without its
+ * env-level part, then k_obstacles (warp per agent: GJK against the env's boxes, then the scan clip) and, with env_level or
+ * start_poses, k_env_tail_obst (thread per env: lap logic, repeat bookkeeping, auto-reset, respawn).  F110_ERR_INVALID before
+ * anything is enqueued for K outside [1, 16], NULL boxes or active, count_min > count_max or count_max > K (or count_min < 0),
+ * a clearance that is negative or not finite, candidate tables that do not match the map's layers, and what the call without
+ * obstacles rejects.  No allocation, no host synchronisation: capturable in a CUDA graph. */
+int f110_step_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                   const double *actions, const f110_obstacles *obst, void *stream);
+int f110_tick_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                   const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                   uint64_t seed, const f110_obstacles *obst, void *stream);
+/* The intermediate ticks run the contact part of k_obstacles alone (their scans do not exist); the march and the marched
+ * subset of the short path are unchanged, since the iTTC check does not see boxes. */
+int f110_tick_repeat_ticks_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                                const double *actions, int32_t repeat, int32_t first_tick, int32_t num_ticks, const f110_repeat *rep,
+                                int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
+                                const f110_obstacles *obst, void *stream);
+/* f110_autoreset, and the respawn of the boxes of every env it restarts (with candidates). */
+int f110_autoreset_obst(const f110_sim *sim, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
+                        uint64_t tick, const f110_obstacles *obst, void *stream);
+/* The respawn draw for the envs whose env_mask byte is non-zero (NULL: all), at tick counter `tick`, after the agents are placed
+ * (a host reset).  For slot k of env e at tick t, with base = seed + 0xA0761D6478BD642F (t+1) + 0xE7037ED1A0B428DB (e+1) (mod
+ * 2^64) and u(h) = (h >> 11) 2^-53:  the active count c = count_min + min(floor(u(mix64(base + 0x589965CC75374CC3)) S), S - 1),
+ * S = count_max - count_min + 1; row j = min(floor(u(mix64(base + 0x8EBC6AF09C88C6E3 (k+1))) C_l), C_l - 1) of the env's table
+ * is copied to the slot; the slot is active iff k < c and dx^2 + dy^2 >= clearance^2 for every agent of the env (positions from
+ * sim->state).  mix64 is the finaliser of the auto-reset's start-pose draw.  The tick's auto-reset uses the tick counter it
+ * draws its start poses with.  F110_ERR_INVALID also without candidates and with more than 32 agents per env. */
+int f110_obstacles_respawn(const f110_sim *sim, const f110_obstacles *obst, const uint8_t *env_mask, uint64_t tick, void *stream);
+
 /* Same tick through HOST buffers: copies actions H2D, runs f110_step (+ f110_env_post_step when the
  * lap arrays are bound), copies the observation D2H and synchronises the stream.
  * Any output pointer may be NULL to skip that copy.  Host buffers should be pinned. */
@@ -358,6 +425,13 @@ int f110_scan_layers(const f110_map *map, const f110_beams *beams, const double 
 int f110_render_views(const f110_sim *sim, const f110_map *map, const int32_t *agent_ids, int32_t V, int32_t height,
                       int32_t width, double metres_per_pixel, double forward_offset, int32_t heading_up, uint8_t *out,
                       void *stream);
+/* f110_render_views with the env's static box obstacles (f110_obstacles) drawn as class 5: every present slot is the quad
+ * get_vertices_cs(x, y, cos, sin, length, width) with (sin, cos) = sincos(yaw), tested as the car quads; priority
+ * 4 > 3 > 5 > 2 > 1 / 0.  obst == NULL is f110_render_views; F110_ERR_INVALID for the structs the _obst tick entry points
+ * reject (the candidate tables are not read). */
+int f110_render_views_obst(const f110_sim *sim, const f110_map *map, const f110_obstacles *obst, const int32_t *agent_ids, int32_t V,
+                           int32_t height, int32_t width, double metres_per_pixel, double forward_offset, int32_t heading_up,
+                           uint8_t *out, void *stream);
 /* vehicle_dynamics_st (dynamic_models.py:123-176): x [M][7], u [M][2], params [18] -> f [M][7]. */
 int f110_vehicle_dynamics_st(const double *x, const double *u, const double *params, int32_t M, double *f,
                              void *stream);
