@@ -91,6 +91,13 @@ class F110Obstacles(C.Structure):
 
 MAX_OBSTACLES = 16
 
+
+class F110Lidar(C.Structure):
+    _fields_ = [('mask', C.c_uint32), ('list', _dp), ('list_count', _dp), ('listed', _dp)]
+
+
+LIDAR_ALL = 0xFFFFFFFF
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol declared
 # in include/f110_b200.h is exported.
 _P = C.POINTER
@@ -125,6 +132,13 @@ SIGNATURES = {
                                               C.c_uint64, _P(F110Obstacles), _dp]),
     'f110_autoreset_obst': (C.c_int, [_P(F110Sim), _dp, C.c_int32, C.c_int32, C.c_uint64, C.c_uint64, _P(F110Obstacles), _dp]),
     'f110_obstacles_respawn': (C.c_int, [_P(F110Sim), _P(F110Obstacles), _dp, C.c_uint64, _dp]),
+    'f110_step_lidar': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, _P(F110Obstacles),
+                                  _P(F110Lidar), _dp]),
+    'f110_tick_lidar': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32, _dp, C.c_int32,
+                                  C.c_int32, C.c_uint64, _P(F110Obstacles), _P(F110Lidar), _dp]),
+    'f110_tick_repeat_ticks_lidar': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32,
+                                               C.c_int32, C.c_int32, _P(F110Repeat), C.c_int32, _dp, C.c_int32, C.c_int32,
+                                               C.c_uint64, _P(F110Obstacles), _P(F110Lidar), _dp]),
     'f110_step_host': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs), _dp]),
     'f110_step_host_async': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110Beams), _dp, _dp, _P(F110HostObs),
                                        _P(F110HostObs), _dp, _dp, _dp, _dp]),

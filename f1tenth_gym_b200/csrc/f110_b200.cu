@@ -20,6 +20,7 @@
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (no FMA contraction).
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
@@ -339,6 +340,93 @@ __global__ void __launch_bounds__(128) k_dynamics(f110_sim s, const double *__re
     ap[0] = st[0]; ap[1] = st[1]; ap[2] = st[4];
     sincos(st[4], ap + 4, ap + 3);
     s.wall_flag[a] = 0;
+}
+
+// ------------------------------------------------------------------------------------ k_lidar_order (f110_lidar)
+// The march queue of a tick with a lidar mask: build_march_order over the items of the agents whose slot has a lidar only.
+// Item w of N * slots * ipa is slice w % ipa of the (w / ipa)-th such agent, envs in order and the slots of an env in ascending
+// order; entries keep the (agent << 8 | slice) encoding, so the march kernels run unchanged.  A launch of its own after
+// k_dynamics (which then has no queue-building blocks): an instance of k_dynamics with a mask-aware builder changes the code of
+// the k_dynamics every tick without a mask runs.  The statements are build_march_order's except where an item's agent is found.
+struct LidarOrder {
+    uint32_t mask;           // bit i: slot i has a lidar (no bit at or above num_agents)
+    unsigned slots;          // popcount of mask, >= 1
+};
+__device__ __forceinline__ unsigned lidar_agent(unsigned r, const LidarOrder &lo, unsigned A) {
+    const unsigned e = r / lo.slots, k = r - e * lo.slots;
+    unsigned m = lo.mask;
+    for (unsigned i = 0; i < k; i++) m &= m - 1u;          // drop the k lowest set bits: the k-th lidar slot is the lowest left
+    return e * A + (unsigned)(__ffs((int)m) - 1);
+}
+__global__ void __launch_bounds__(128) k_lidar_order(f110_sim s, LidarOrder lo) {
+    __shared__ unsigned s_cnt[3], s_base[3];
+    const unsigned items = (unsigned)s.num_envs * lo.slots * (unsigned)s.march_ipa;
+    const unsigned A = (unsigned)s.num_agents;
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned ipa = (unsigned)s.march_ipa;
+    if (threadIdx.x < 3) s_cnt[threadIdx.x] = 0u;
+    const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned w0 = t * F110_ORDER_ITEMS_PER_THREAD;
+    unsigned packed[F110_ORDER_ITEMS_PER_THREAD], c[F110_ORDER_ITEMS_PER_THREAD + 2];
+    int cls[F110_ORDER_ITEMS_PER_THREAD];
+    unsigned a = 0, j = 0, r = 0;
+    if (w0 < items) { r = w0 / ipa; j = w0 - r * ipa; a = lidar_agent(r, lo, A); }
+    c[0] = (w0 < items && j > 0) ? s.march_cost[((a << 8) | j) - 1u] : F110_Q_UNKNOWN;
+    unsigned aa = a, jj = j;
+#pragma unroll
+    for (int k = 0; k < F110_ORDER_ITEMS_PER_THREAD; k++) {
+        const bool live = w0 + (unsigned)k < items;
+        packed[k] = (aa << 8) | jj;
+        c[k + 1] = live ? s.march_cost[packed[k]] : F110_Q_UNKNOWN;
+        cls[k] = live ? 0 : -1;
+        if (++jj == ipa) { jj = 0; aa = lidar_agent(++r, lo, A); }
+    }
+    {
+        const unsigned wl = w0 + F110_ORDER_ITEMS_PER_THREAD;
+        c[F110_ORDER_ITEMS_PER_THREAD + 1] = (wl < items && jj > 0) ? s.march_cost[(aa << 8) | jj] : F110_Q_UNKNOWN;
+    }
+    unsigned mine = 0u;
+#pragma unroll
+    for (int k = 0; k < F110_ORDER_ITEMS_PER_THREAD; k++) {
+        if (cls[k] == 0) {
+            const unsigned sj = packed[k] & 255u;
+            unsigned m = c[k + 1];
+            if (m != F110_Q_UNKNOWN) {
+                if (sj > 0 && c[k] != F110_Q_UNKNOWN) m = max(m, c[k]);
+                if (sj + 1 < ipa && c[k + 2] != F110_Q_UNKNOWN) m = max(m, c[k + 2]);
+            }
+            cls[k] = (c[k + 1] == F110_Q_UNKNOWN || c[k + 1] >= F110_Q_VERY_HEAVY) ? 0 : (m >= F110_Q_HEAVY) ? 1 : 2;
+            mine += 1u << (10 * cls[k]);
+        }
+    }
+    unsigned incl = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned v = __shfl_up_sync(0xffffffffu, incl, o);
+        if ((int)lane >= o) incl += v;
+    }
+    const unsigned excl = incl - mine;
+    const unsigned wtot = __shfl_sync(0xffffffffu, incl, 31);
+    __syncthreads();
+    unsigned wbase = 0u;
+    if (lane < 3u) {
+        const unsigned n = (wtot >> (10 * lane)) & 1023u;
+        wbase = n ? atomicAdd(&s_cnt[lane], n) : 0u;
+    }
+    const unsigned b0 = __shfl_sync(0xffffffffu, wbase, 0), b1 = __shfl_sync(0xffffffffu, wbase, 1),
+                   b2 = __shfl_sync(0xffffffffu, wbase, 2);
+    __syncthreads();
+    if (threadIdx.x < 3) s_base[threadIdx.x] = s_cnt[threadIdx.x] ? atomicAdd(s.march_count + threadIdx.x, s_cnt[threadIdx.x]) : 0u;
+    __syncthreads();
+    unsigned pos[3] = { s_base[0] + b0 + (excl & 1023u), s_base[1] + b1 + ((excl >> 10) & 1023u),
+                        s_base[2] + b2 + ((excl >> 20) & 1023u) };
+#pragma unroll
+    for (int k = 0; k < F110_ORDER_ITEMS_PER_THREAD; k++) {
+        if (cls[k] >= 0) {
+            const unsigned at = (cls[k] == 0) ? pos[0]++ : (cls[k] == 1) ? pos[1]++ : pos[2]++;
+            if (at < items) s.march_order[(size_t)cls[k] * items + at] = packed[k];
+        }
+    }
 }
 
 // ------------------------------------------------------------------------------------ k_raymarch
@@ -951,6 +1039,111 @@ __global__ void __launch_bounds__(F110_TAIL_NOSCAN_THREADS) k_tail_noscan(f110_s
     }
 }
 
+// ------------------------------------------------------------------------------------ k_lidar_cast (f110_lidar)
+// The opponent ray-cast of a tick with a lidar mask, for the egos whose slot has a lidar: a warp per such ego (LidarOrder's
+// enumeration), any A <= 32.  Lane oj < A - 1 does k_tail2's scalar prologue for opponent oj into the warp's task records,
+// then the warp walks its opponents in ascending order with k_tail2's beam loop -- the same statements, so the scans are
+// bit-identical to the plain tick's (blocked_view_indices_cs equals the warp-cooperative version of k_tail / k_finalize).
+// It must run before k_tail_noscan: that kernel's auto-reset clears wall_flag, which gives the yaw an iTTC hit zeroed.
+// Thread 0 of block 0 consumes the march queue counters, as the tails' end_of_tick_housekeeping does.
+#define F110_LIDAR_CAST_WARPS 4
+__global__ void __launch_bounds__(32 * F110_LIDAR_CAST_WARPS) k_lidar_cast(f110_sim s, BeamView bv, LidarOrder lo,
+                                                                            double max_scan_range) {
+    __shared__ TailTask tasks_all[F110_LIDAR_CAST_WARPS][31];
+    const int A = s.num_agents;
+    const int opp = A - 1;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (blockIdx.x == 0 && threadIdx.x == 0) end_of_tick_housekeeping(s);
+    const unsigned r = blockIdx.x * F110_LIDAR_CAST_WARPS + (unsigned)warp;
+    if (opp < 1 || r >= (unsigned)s.num_envs * lo.slots) return;       // warp-uniform
+    const int a = (int)lidar_agent(r, lo, (unsigned)A);
+    const int env = a / A, slot = a - env * A;
+    TailTask *tasks = tasks_all[warp];
+    const int hit = s.wall_flag[a];
+    const double *pa = s.agent_poses + 5 * (size_t)a;
+    const double px = pa[0], py = pa[1];
+    // check_ttc zeroes state[3:] -- including the yaw -- before the opponent ray-cast reads it (:246-249, :225)
+    const double yaw = hit ? 0.0 : pa[2];
+    const double cyaw = hit ? 1.0 : pa[3], syaw = hit ? 0.0 : pa[4];
+    const double *p = s.params + (size_t)(s.params_per_env ? a : slot) * F110_NPARAM;
+    const double length = p[P_LENGTH], width = p[P_WIDTH];
+    const double half_diag = 0.5 * sqrt(length * length + width * width);
+    if (lane < opp) {
+        const int oj = lane, j = oj < slot ? oj : oj + 1;     // opponents in ascending index, skipping the ego itself
+        const double *pb = s.agent_poses + 5 * (size_t)(env * A + j);
+        TailTask &k = tasks[oj];
+        const double ddx = pb[0] - px, ddy = pb[1] - py;
+        const double far = max_scan_range + half_diag;
+        int active = 1;
+        if (ddx * ddx + ddy * ddy > far * far) active = 0;     // cannot shorten any beam (see finalize_agent)
+        k.active = active;
+        if (active) {
+            double v[8];
+            get_vertices_cs(pb[0], pb[1], pb[3], pb[4], length, width, v);
+            int lo_i, hi_i;
+            double phi;
+            blocked_view_indices_cs(px, py, cyaw, syaw, v, bv.scan_angles, bv.num_beams, bv.fov, bv.angle_increment, pb[0], pb[1],
+                                    lo_i, hi_i, phi);
+            double cone = 4.0;
+            if (hi_i - lo_i >= 96) {
+                const double dist = sqrt(ddx * ddx + ddy * ddy);
+                if (dist > 1.25 * half_diag) cone = asin(half_diag / dist) + 0.05;
+            }
+            k.px = px; k.py = py; k.yaw = yaw; k.phi = phi; k.cone = cone; k.lo = lo_i; k.hi = hi_i;
+#pragma unroll
+            for (int q = 0; q < 8; q++) k.v[q] = v[q];
+        }
+    }
+    __syncwarp();
+    float *scan = s.scans + (size_t)a * bv.num_beams;
+    for (int oj = 0; oj < opp; oj++) {
+        const TailTask &k = tasks[oj];
+        if (!k.active) continue;
+        const double kpx = k.px, kpy = k.py, kyaw = k.yaw, phi = k.phi, cone = k.cone;
+        const int lo_i = k.lo, hi_i = k.hi;
+        double v[8];
+#pragma unroll
+        for (int q = 0; q < 8; q++) v[q] = k.v[q];
+        auto cast_beams = [&](int i0, int i1) {
+            for (int i = i0 + lane; i <= i1; i += 32) {
+                const float cur = scan[i];
+                double bt = kyaw + bv.scan_angles[i];
+                double dl = bt - phi;
+                dl = dl - (2 * M_PI) * rint(dl * (1.0 / (2 * M_PI)));
+                const double adl = fabs(dl);
+                if (adl > cone && (M_PI - adl) > cone) continue;
+                double v3x, v3y;
+                sincos(bt + M_PI / 2., &v3y, &v3x);
+                const double curd = (double)cur;
+                double rr = INFINITY;
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    int e2 = (e + 1) & 3;
+                    double d = get_range_below(kpx, kpy, v3x, v3y, v[2 * e], v[2 * e + 1], v[2 * e2], v[2 * e2 + 1], curd);
+                    if (d < rr) rr = d;
+                }
+                float rf = (float)rr;
+                if (rf < cur) scan[i] = rf;
+            }
+        };
+        if (cone < 3.5 && hi_i - lo_i >= 96) {
+            const double base = wrap_2pi_diff(phi - kyaw), half = bv.fov / 2., inv_inc = 1.0 / bv.angle_increment;   // (see finalize_agent)
+            const int m0 = max(-3, (int)floor((-half - cone - 0.02 - base) * (1.0 / M_PI))),
+                      m1 = min(5, (int)ceil((half + cone + 0.02 - base) * (1.0 / M_PI)));
+            for (int m = m0; m <= m1; m++) {
+                const double c = base + (double)m * M_PI;
+                const double f0 = (c - cone + half) * inv_inc - 2.0, f1 = (c + cone + half) * inv_inc + 2.0;
+                if (f1 < (double)lo_i || f0 > (double)hi_i) continue;
+                const int i0 = max(lo_i, (int)floor(fmax(f0, (double)lo_i))), i1 = min(hi_i, (int)ceil(fmin(f1, (double)hi_i)));
+                cast_beams(i0, i1);
+            }
+        } else {
+            cast_beams(lo_i, hi_i);
+        }
+        __syncwarp();
+    }
+}
+
 }  // namespace f110
 #include "obstacles.cuh"     // k_obstacles, k_env_tail_obst: built on the tail's device functions above
 namespace f110 {
@@ -1266,10 +1459,12 @@ struct MarchPlan {
     MarchQueue mq;
 };
 
+// queued_agents: the agents whose items the queue holds, -1 = all (a tick with a lidar mask queues the slots that have a lidar only)
 static int plan_march(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
-                      const MapGeom &geom, int variant, MarchPlan *plan) {
+                      const MapGeom &geom, int variant, MarchPlan *plan, long long queued_agents = -1) {
     MarchPlan p = {};
     const int NA = sim->num_envs * sim->num_agents;
+    const long long QA = queued_agents < 0 ? (long long)NA : queued_agents;
     const unsigned sms = (unsigned)num_sms();
     p.variant = variant;
     p.noise = sim->noise_std > 0.0; p.count = sim->lookup_counter != nullptr;
@@ -1306,7 +1501,7 @@ static int plan_march(const f110_sim *sim, const f110_map *map, const f110_march
     if (geom.het && (!p.lean || tile || !p.layered)) return F110_ERR_INVALID;
     p.dyn_blocks = (NA + 127) / 128;
     p.order_blocks = tile ? p.dyn_blocks
-                   : queued ? (int)(((long long)NA * sim->march_ipa + 128 * F110_ORDER_ITEMS_PER_THREAD - 1) / (128 * F110_ORDER_ITEMS_PER_THREAD))
+                   : queued ? (int)((QA * sim->march_ipa + 128 * F110_ORDER_ITEMS_PER_THREAD - 1) / (128 * F110_ORDER_ITEMS_PER_THREAD))
                    : 0;
     p.agent_queue = tile ? 1 : 0;
 
@@ -1332,7 +1527,7 @@ static int plan_march(const f110_sim *sim, const f110_map *map, const f110_march
 
     MarchQueue &mq = p.mq;
     mq.cost = sim->march_cost; mq.order = sim->march_order; mq.count = sim->march_count;
-    mq.ipa = (unsigned)sim->march_ipa; mq.items = (unsigned)NA * mq.ipa;
+    mq.ipa = (unsigned)sim->march_ipa; mq.items = (unsigned)QA * mq.ipa;
     mq.chunk_shift = march_chunk();
     mq.claim = sim->march_count + 3;
     // Dynamic tail of the queue (k_march_lean<DYN>): g_dyn_pct % of every block's share is dealt statically.  Whether the tail
@@ -1835,8 +2030,9 @@ struct TailOpts {
 };
 // what launch_tail launched, for the launch record
 struct TailShape {
-    enum { TAIL2, TAIL, FINALIZE } kernel;
+    enum { TAIL2, TAIL, FINALIZE, NOSCAN } kernel;
     int epb, threads, grid;          // envs per block, block size, blocks
+    int cast_grid;                   // NOSCAN (a tick with a lidar mask): blocks of k_lidar_cast before k_tail_noscan
     size_t smem;                     // TAIL2
     int lb_threads, lb_minb;         // TAIL: the launch bounds of the instance
     bool separate;                   // FINALIZE standing in for the fused tail (more than 32 agents per env)
@@ -1966,6 +2162,10 @@ static void write_launch_record(const MarchPlan &p, const MapGeom &geom, const f
     case TailShape::FINALIZE:
         snprintf(tail, sizeof(tail), "tail=k_finalize%s epb=0 threads=128 tail_grid=%d", ts.separate ? "+separate" : "", ts.grid);
         break;
+    case TailShape::NOSCAN:
+        snprintf(tail, sizeof(tail), "tail=k_lidar_cast+k_tail_noscan cast_grid=%d epb=%d threads=%d tail_grid=%d", ts.cast_grid,
+                 ts.epb, ts.threads, ts.grid);
+        break;
     }
     snprintf(g_launch_rec, sizeof(g_launch_rec), "%s%s%s static_runs=%u per_warp=%u %s", march, geom.het ? "" : " HET=0",
              p.rot && p.lean ? "" : " ROT=0", p.mq.static_runs, p.per_warp, tail);
@@ -1982,7 +2182,7 @@ static int plan_obstacles(const f110_sim *sim, const f110_obstacles *o, int num_
     if (o->per_env < 1 || o->per_env > F110_MAX_OBSTACLES || !o->boxes || !o->active) return F110_ERR_INVALID;
     if (o->count_min < 0 || o->count_min > o->count_max || o->count_max > o->per_env) return F110_ERR_INVALID;
     if (!(o->clearance >= 0.0) || !isfinite(o->clearance)) return F110_ERR_INVALID;
-    p->k.boxes = o->boxes; p->k.active = o->active; p->k.hit = o->hit; p->k.K = o->per_env;
+    p->k.boxes = o->boxes; p->k.active = o->active; p->k.hit = o->hit; p->k.K = o->per_env; p->k.lidar = F110_LIDAR_ALL;
     ObstDraw &d = p->d;
     memset(&d, 0, sizeof(d));
     d.boxes = o->boxes; d.active = o->active; d.cand = o->candidates; d.K = o->per_env;
@@ -2006,12 +2206,17 @@ static int plan_obstacles(const f110_sim *sim, const f110_obstacles *o, int num_
 static cudaEvent_t g_obst_ev[3] = {nullptr, nullptr, nullptr};
 // after the tail of a tick that ran without its env-level part: k_obstacles, then (a tick with lap logic or auto-reset)
 // k_env_tail_obst.  tail NULL: f110_step.  rd: the repeat bookkeeping of an intermediate tick of f110_tick_repeat, or NULL.
+// lidar: the mask of a tick with a lidar mask on its short path (only those slots' scans are clipped), else F110_LIDAR_ALL
 static int launch_obst_tail(const f110_sim *sim, const BeamView &bv, const ObstPlan &ob, const TailOpts *tail, bool scan,
-                            const RepeatDone *rd, double max_scan, cudaStream_t st) {
+                            const RepeatDone *rd, double max_scan, cudaStream_t st, uint32_t lidar = F110_LIDAR_ALL) {
     const int NA = sim->num_envs * sim->num_agents;
     const unsigned grid = (unsigned)(((long long)NA * 32 + 127) / 128);
     if (g_obst_ev[0]) CUDA_TRY(cudaEventRecord(g_obst_ev[0], st));
-    if (scan) k_obstacles<true><<<grid, 128, 0, st>>>(*sim, bv, ob.k, max_scan);
+    if (scan && lidar != F110_LIDAR_ALL) {
+        ObstK k = ob.k;
+        k.lidar = lidar;
+        k_obstacles<true, true><<<grid, 128, 0, st>>>(*sim, bv, k, max_scan);
+    } else if (scan) k_obstacles<true><<<grid, 128, 0, st>>>(*sim, bv, ob.k, max_scan);
     else k_obstacles<false><<<grid, 128, 0, st>>>(*sim, bv, ob.k, max_scan);
     LAUNCH_CHECK("k_obstacles");
     if (g_obst_ev[1]) CUDA_TRY(cudaEventRecord(g_obst_ev[1], st));
@@ -2026,27 +2231,92 @@ static int launch_obst_tail(const f110_sim *sim, const BeamView &bv, const ObstP
 }
 
 // ------------------------------------------------------------------------------------ the plan and the launches of a tick
+// ---- ticks whose scans nobody reads, in whole (the intermediate ticks of f110_tick_repeat) or in part (the sensorless agents of
+// a tick with a lidar mask): march_ttc.cuh.  Decided here from what the host can observe, never by an option.  The short path
+// needs: no scan noise (the bound does not hold for a Gaussian, and the Philox stream must stay the plain run's); a lean march
+// family, which brings the per-agent record, the doubled LUT and `dt_min_positive > eps`; a known max side distance below
+// max_range (otherwise every moving agent is listed); and at most 32 agents per env (the block-owns-envs tail).
+static bool ttc_path_ok(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const MarchPlan &m) {
+    const bool lean_family = m.family == MarchFamily::LEAN || m.family == MarchFamily::LEAN_BRICK || m.family == MarchFamily::LEAN_HET ||
+                             m.family == MarchFamily::LEAN_HET_RES || m.family == MarchFamily::LEAN_ROT;
+    return sim->noise_std == 0.0 && m.lean && lean_family && sim->march_rec && map->sincos2 && map->dt_min_positive > map->eps &&
+           beams->side_max > 0.0 && beams->side_max < map->max_range && sim->num_agents <= 32;
+}
+template <int UNITS>
+static int ttc_grid(bool count, unsigned *grid) {
+    static int per_sm[2] = {0, 0};
+    int &n = per_sm[count ? 1 : 0];
+    if (n <= 0) {
+        if (count) CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, true>, F110_TTC_THREADS, 0));
+        else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, false>, F110_TTC_THREADS, 0));
+        if (n <= 0) return F110_ERR_INVALID;
+    }
+    *grid = (unsigned)n * (unsigned)num_sms();
+    return F110_OK;
+}
+// k_march_ttc's units (F110_SCAN_UNITS_*) for the tick's march, and its fixed grid: resident blocks per SM x SMs
+static int plan_ttc(const MarchPlan &m, int *units, unsigned *grid) {
+    *units = m.rot ? F110_SCAN_UNITS_ROT : m.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+    return *units == F110_SCAN_UNITS_ROT ? ttc_grid<F110_SCAN_UNITS_ROT>(m.count, grid)
+         : *units == F110_SCAN_UNITS_CELLS ? ttc_grid<F110_SCAN_UNITS_CELLS>(m.count, grid)
+                                           : ttc_grid<F110_SCAN_UNITS_METRES>(m.count, grid);
+}
+
 struct TickPlan {
     MapGeom geom;
     MarchPlan march;
     const ObstPlan *obst;    // NULL: no obstacles (the tail runs as before)
+    // a lidar mask (f110_lidar): on the short path `lidar` is set, the march plan queues the `lidar_slots` slots that have a
+    // lidar, and k_march_ttc runs with ttc_units / ttc_grid; lidar_full: a mask was given and is ignored (the full path)
+    const f110_lidar *lidar;
+    bool lidar_full;
+    unsigned lidar_slots;
+    int ttc_units;
+    unsigned ttc_grid;
 };
+// a lidar mask the call may take (before anything is enqueued, on either path); sim already checked
+static int check_lidar(const f110_sim *sim, const f110_lidar *lidar) {
+    if (!lidar || lidar->mask == F110_LIDAR_ALL) return F110_OK;
+    if (sim->num_agents > 32) return F110_ERR_INVALID;
+    if (sim->num_agents < 32 && (lidar->mask >> sim->num_agents) != 0u) return F110_ERR_INVALID;
+    if (!lidar->list || !lidar->list_count) return F110_ERR_INVALID;
+    return F110_OK;
+}
 static int plan_tick(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
-                     const double *actions, TickPlan *tp) {
+                     const double *actions, TickPlan *tp, const f110_lidar *lidar = nullptr) {
     int rc;
     tp->obst = nullptr;
-    if ((rc = check_sim(sim)) || (rc = check_map(map)) || (rc = check_beams(beams))) return rc;
+    tp->lidar = nullptr; tp->lidar_full = false; tp->lidar_slots = 0u; tp->ttc_units = 0; tp->ttc_grid = 0u;
+    if ((rc = check_sim(sim)) || (rc = check_lidar(sim, lidar)) || (rc = check_map(map)) || (rc = check_beams(beams))) return rc;
     if (!actions) return F110_ERR_INVALID;
     if (sim->lookup_counter && sim->noise_std > 0.0) return F110_ERR_INVALID;   // counting runs are noise-free by construction
     if ((long long)sim->num_envs * sim->num_agents > 0x7fffffffll) return F110_ERR_INVALID;
     if ((rc = classify_map(map, &tp->geom))) return rc;
-    return plan_march(sim, map, tables, beams, tp->geom, rm_variant(), &tp->march);
+    if ((rc = plan_march(sim, map, tables, beams, tp->geom, rm_variant(), &tp->march))) return rc;
+    if (!lidar || lidar->mask == F110_LIDAR_ALL) return F110_OK;
+    if (!ttc_path_ok(sim, map, beams, tp->march)) { tp->lidar_full = true; return F110_OK; }
+    tp->lidar = lidar;
+    tp->lidar_slots = (unsigned)__builtin_popcount(lidar->mask);
+    // the same family and kernel shape rules on the shorter queue (the family never depends on the queue length)
+    if ((rc = plan_march(sim, map, tables, beams, tp->geom, rm_variant(), &tp->march, (long long)sim->num_envs * tp->lidar_slots)))
+        return rc;
+    return plan_ttc(tp->march, &tp->ttc_units, &tp->ttc_grid);
+}
+static int launch_lidar_tick(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                             const double *actions, TickPlan &tp, cudaStream_t st, const TailOpts *tail);
+static void append_launch_record(const char *fmt, ...) {
+    const size_t n = strlen(g_launch_rec);
+    va_list va;
+    va_start(va, fmt);
+    vsnprintf(g_launch_rec + n, sizeof(g_launch_rec) - n, fmt, va);
+    va_end(va);
 }
 static int launch_tick(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                        const double *actions, TickPlan &tp, cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail) {
     int rc;
     MarchPlan &plan = tp.march;
     const bool pdl = (ev == nullptr);         // PDL only when no events are recorded between the kernels
+    if (tp.lidar) return launch_lidar_tick(sim, map, tables, beams, actions, tp, st, tail);
 
     if (ev) CUDA_TRY(cudaEventRecord(ev[0], st));
     k_dynamics<<<plan.dyn_blocks + plan.order_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, plan.dyn_blocks,
@@ -2061,66 +2331,44 @@ static int launch_tick(const f110_sim *sim, const f110_map *map, const f110_marc
     if ((rc = launch_tail(sim, map, bv, tp.obst ? nullptr : tail, pdl && plan.lean, st, &ts))) return rc;
     if (tp.obst && (rc = launch_obst_tail(sim, bv, *tp.obst, tail, true, nullptr, max_scan_range(sim, map), st))) return rc;
     write_launch_record(plan, tp.geom, map, ts);
-    if (tp.obst) {
-        const size_t n = strlen(g_launch_rec);
-        snprintf(g_launch_rec + n, sizeof(g_launch_rec) - n, " obst=%d", tp.obst->k.K);
-    }
+    if (tp.obst) append_launch_record(" obst=%d", tp.obst->k.K);
+    if (tp.lidar_full) append_launch_record(" lidar=full");
     if (ev) CUDA_TRY(cudaEventRecord(ev[3], st));
     return F110_OK;
 }
 // ---- f110_tick_repeat: `repeat` ticks under one action; the ticks whose scans nobody reads march only for the iTTC flag
-// The plan of the call: the plain tick's plan, and whether ticks 0 .. repeat - 2 take the short path (march_ttc.cuh).  Decided
-// here from what the host can observe, never by an option.  The short path needs: no scan noise (the bound does not hold for
-// a Gaussian, and the Philox stream must stay the plain run's); a lean march family, which brings the per-agent record, the
-// doubled LUT and `dt_min_positive > eps`; a known max side distance below max_range (otherwise every moving agent is
-// listed); and at most 32 agents per env (the block-owns-envs tail).  Everything else runs `repeat` plain ticks.
+// The plan of the call: the plain tick's plan, and whether ticks 0 .. repeat - 2 take the short path (ttc_path_ok).
+// Everything else runs `repeat` plain ticks.
 struct RepeatPlan {
     TickPlan tick;
     bool ttc;                // ticks 0 .. repeat - 2: k_dynamics, k_ttc_select, k_march_ttc, k_tail_noscan
     int units;               // F110_SCAN_UNITS_* of k_march_ttc
     unsigned grid;           // its fixed grid: resident blocks per SM x SMs
 };
-template <int UNITS>
-static int ttc_grid(bool count, unsigned *grid) {
-    static int per_sm[2] = {0, 0};
-    int &n = per_sm[count ? 1 : 0];
-    if (n <= 0) {
-        if (count) CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, true>, F110_TTC_THREADS, 0));
-        else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, false>, F110_TTC_THREADS, 0));
-        if (n <= 0) return F110_ERR_INVALID;
-    }
-    *grid = (unsigned)n * (unsigned)num_sms();
-    return F110_OK;
-}
 static int plan_repeat(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                        const double *actions, int32_t repeat, RepeatPlan *rp) {
     int rc;
     if ((rc = plan_tick(sim, map, tables, beams, actions, &rp->tick))) return rc;
     const MarchPlan &m = rp->tick.march;
-    const bool lean_family = m.family == MarchFamily::LEAN || m.family == MarchFamily::LEAN_BRICK || m.family == MarchFamily::LEAN_HET ||
-                             m.family == MarchFamily::LEAN_HET_RES || m.family == MarchFamily::LEAN_ROT;
-    rp->ttc = repeat > 1 && sim->noise_std == 0.0 && m.lean && lean_family && sim->march_rec && map->sincos2 &&
-              map->dt_min_positive > map->eps && beams->side_max > 0.0 && beams->side_max < map->max_range && sim->num_agents <= 32;
+    rp->ttc = repeat > 1 && ttc_path_ok(sim, map, beams, m);
     rp->units = m.rot ? F110_SCAN_UNITS_ROT : m.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
     rp->grid = 0u;
     if (!rp->ttc) return F110_OK;
-    const bool count = m.count;
-    return rp->units == F110_SCAN_UNITS_ROT ? ttc_grid<F110_SCAN_UNITS_ROT>(count, &rp->grid)
-         : rp->units == F110_SCAN_UNITS_CELLS ? ttc_grid<F110_SCAN_UNITS_CELLS>(count, &rp->grid)
-                                              : ttc_grid<F110_SCAN_UNITS_METRES>(count, &rp->grid);
+    return plan_ttc(m, &rp->units, &rp->grid);
 }
 
-static TtcK fill_ttc_k(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const RepeatPlan &rp, const f110_repeat *rep,
-                       int tick) {
-    const MarchPlan &m = rp.tick.march;
-    const bool het = rp.tick.geom.het;
+// list / count: the agents k_ttc_select listed
+static TtcK fill_ttc_k(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const TickPlan &tp, const uint32_t *list,
+                       const uint32_t *count) {
+    const MarchPlan &m = tp.march;
+    const bool het = tp.geom.het;
     TtcK q;
     q.table = m.cell_units ? map->dt_cells_pad : map->dt;
     q.dt = map->dt;
     q.sincos2 = reinterpret_cast<const double2 *>(map->sincos2);
     q.cos_side = reinterpret_cast<const double2 *>(beams->cos_side);
     q.rec = reinterpret_cast<const double2 *>(sim->march_rec);
-    q.list = rep->list; q.count = rep->list_count + tick;
+    q.list = list; q.count = count;
     q.wall_flag = sim->wall_flag; q.lookup_counter = sim->lookup_counter;
     q.layer_geom = het ? map->layer_geom : nullptr; q.layer_res = het ? map->layer_res : nullptr;
     q.layer_rot = het ? map->layer_rot : nullptr; q.env_layer = het ? sim->env_layer : nullptr;
@@ -2148,6 +2396,11 @@ static void launch_march_ttc_t(const TtcK &q, bool count, unsigned grid, cudaStr
     if (count) k_march_ttc<UNITS, true><<<grid, F110_TTC_THREADS, 0, st>>>(q);
     else k_march_ttc<UNITS, false><<<grid, F110_TTC_THREADS, 0, st>>>(q);
 }
+static void launch_march_ttc(const TtcK &q, int units, bool count, unsigned grid, cudaStream_t st) {
+    if (units == F110_SCAN_UNITS_ROT) launch_march_ttc_t<F110_SCAN_UNITS_ROT>(q, count, grid, st);
+    else if (units == F110_SCAN_UNITS_CELLS) launch_march_ttc_t<F110_SCAN_UNITS_CELLS>(q, count, grid, st);
+    else launch_march_ttc_t<F110_SCAN_UNITS_METRES>(q, count, grid, st);
+}
 
 // one intermediate tick of the short path
 static int launch_ttc_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
@@ -2161,13 +2414,10 @@ static int launch_ttc_tick(const f110_sim *sim, const f110_map *map, const f110_
     TtcSelectK sel;
     sel.rec = reinterpret_cast<const double2 *>(sim->march_rec); sel.list = rep->list; sel.count = rep->list_count + tick;
     sel.marched = rep->marched_agents; sel.d0_scale = m.cell_units ? map->resolution : 1.0; sel.max_range = map->max_range;
-    sel.agents = (unsigned)NA;
+    sel.agents = (unsigned)NA; sel.skip = 0u; sel.num_agents = (unsigned)sim->num_agents;
     k_ttc_select<<<(NA + F110_TTC_SELECT_THREADS - 1) / F110_TTC_SELECT_THREADS, F110_TTC_SELECT_THREADS, 0, st>>>(sel);
     LAUNCH_CHECK("k_ttc_select");
-    const TtcK q = fill_ttc_k(sim, map, beams, rp, rep, tick);
-    if (rp.units == F110_SCAN_UNITS_ROT) launch_march_ttc_t<F110_SCAN_UNITS_ROT>(q, m.count, rp.grid, st);
-    else if (rp.units == F110_SCAN_UNITS_CELLS) launch_march_ttc_t<F110_SCAN_UNITS_CELLS>(q, m.count, rp.grid, st);
-    else launch_march_ttc_t<F110_SCAN_UNITS_METRES>(q, m.count, rp.grid, st);
+    launch_march_ttc(fill_ttc_k(sim, map, beams, rp.tick, rep->list, rep->list_count + tick), rp.units, m.count, rp.grid, st);
     LAUNCH_CHECK("k_march_ttc");
     const int epb = std::max(1, F110_TAIL_NOSCAN_THREADS / sim->num_agents);
     RepeatDone rd;
@@ -2181,6 +2431,85 @@ static int launch_ttc_tick(const f110_sim *sim, const f110_map *map, const f110_
     }
     k_tail_noscan<<<(sim->num_envs + epb - 1) / epb, F110_TAIL_NOSCAN_THREADS, 0, st>>>(*sim, (int)tail.env_level, tail.ar, epb, rd);
     LAUNCH_CHECK("k_tail_noscan");
+    return F110_OK;
+}
+
+// A tick with a lidar mask on its short path (TickPlan.lidar): S = lidar_slots slots have a lidar.
+//   k_dynamics         the dynamics of every agent, without its queue-building blocks
+//   k_lidar_order      the march queue of the S slots only (skipped when S = 0)
+//   the planned march  unchanged kernels on that queue: scans and iTTC flags of the agents that have a lidar (skipped when S = 0)
+//   k_ttc_select       the sensorless agents a wall could stop, into f110_lidar.list
+//   k_march_ttc        those agents, for the iTTC flag alone
+//   k_lidar_cast       the opponent ray-cast of the egos that have a lidar, and the queue counters (skipped when S = 0)
+//   k_tail_noscan      agent duties, env level and auto-reset -- after the ray-cast, whose yaw comes from wall_flag
+// With obstacles, k_tail_noscan runs without its env level, then k_obstacles<true, true> (contact for every agent, the scan
+// clip for the agents that have a lidar) and k_env_tail_obst.
+static int launch_lidar_tick(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                             const double *actions, TickPlan &tp, cudaStream_t st, const TailOpts *tail) {
+    int rc;
+    MarchPlan &plan = tp.march;
+    const f110_lidar &ld = *tp.lidar;
+    const unsigned S = tp.lidar_slots;
+    const int NA = sim->num_envs * sim->num_agents;
+    const LidarOrder lo = {ld.mask, S};
+    k_dynamics<<<plan.dyn_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, plan.dyn_blocks,
+                                                fill_first_lookup(sim, map, beams, tp.geom, plan));
+    LAUNCH_CHECK("k_dynamics");
+    if (S) {
+        k_lidar_order<<<plan.order_blocks, 128, 0, st>>>(*sim, lo);
+        LAUNCH_CHECK("k_lidar_order");
+    }
+    if (S && (rc = launch_march_plan(plan, sim, map, tables, beams, tp.geom, false, st))) return rc;
+    CUDA_TRY(cudaMemsetAsync(ld.list_count, 0, sizeof(uint32_t), st));
+    TtcSelectK sel;
+    sel.rec = reinterpret_cast<const double2 *>(sim->march_rec); sel.list = ld.list; sel.count = ld.list_count;
+    sel.marched = ld.listed; sel.d0_scale = plan.cell_units ? map->resolution : 1.0; sel.max_range = map->max_range;
+    sel.agents = (unsigned)NA; sel.skip = ld.mask; sel.num_agents = (unsigned)sim->num_agents;
+    k_ttc_select<<<(NA + F110_TTC_SELECT_THREADS - 1) / F110_TTC_SELECT_THREADS, F110_TTC_SELECT_THREADS, 0, st>>>(sel);
+    LAUNCH_CHECK("k_ttc_select");
+    launch_march_ttc(fill_ttc_k(sim, map, beams, tp, ld.list, ld.list_count), tp.ttc_units, plan.count, tp.ttc_grid, st);
+    LAUNCH_CHECK("k_march_ttc");
+    const BeamView bv = make_view(beams);
+    const double max_scan = max_scan_range(sim, map);
+    unsigned cast_grid = 0u;
+    if (S) {
+        cast_grid = (unsigned)(((unsigned long long)sim->num_envs * S + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS);
+        k_lidar_cast<<<cast_grid, 32 * F110_LIDAR_CAST_WARPS, 0, st>>>(*sim, bv, lo, max_scan);
+        LAUNCH_CHECK("k_lidar_cast");
+    }
+    const int epb = std::max(1, F110_TAIL_NOSCAN_THREADS / sim->num_agents);
+    const unsigned tgrid = (unsigned)((sim->num_envs + epb - 1) / epb);
+    RepeatDone rd;
+    rd.done_any = nullptr; rd.done_tick = nullptr; rd.tick = 0;
+    AutoResetArgs ar;
+    memset(&ar, 0, sizeof(ar));
+    if (tail) ar = tail->ar;
+    const int env_level = tail ? (int)tail->env_level : 0;
+    if (tp.obst) {
+        AutoResetArgs no_ar = ar;
+        no_ar.start_poses = nullptr;
+        k_tail_noscan<<<tgrid, F110_TAIL_NOSCAN_THREADS, 0, st>>>(*sim, 0, no_ar, epb, rd);
+        LAUNCH_CHECK("k_tail_noscan");
+        if ((rc = launch_obst_tail(sim, bv, *tp.obst, tail, true, nullptr, max_scan, st, ld.mask))) return rc;
+    } else {
+        k_tail_noscan<<<tgrid, F110_TAIL_NOSCAN_THREADS, 0, st>>>(*sim, env_level, ar, epb, rd);
+        LAUNCH_CHECK("k_tail_noscan");
+    }
+    // the record: the march (when one ran), then the tail kernels
+    g_launch_rec[0] = '\0';
+    if (S) {
+        TailShape ts = {};
+        ts.kernel = TailShape::NOSCAN; ts.epb = epb; ts.threads = F110_TAIL_NOSCAN_THREADS; ts.grid = (int)tgrid;
+        ts.cast_grid = (int)cast_grid;
+        write_launch_record(plan, tp.geom, map, ts);
+    } else {
+        snprintf(g_launch_rec, sizeof(g_launch_rec), "march=none tail=k_tail_noscan epb=%d threads=%d tail_grid=%d", epb,
+                 F110_TAIL_NOSCAN_THREADS, (int)tgrid);
+    }
+    append_launch_record(" ttc=%s grid=%u", tp.ttc_units == F110_SCAN_UNITS_ROT ? "rot" : tp.ttc_units == F110_SCAN_UNITS_CELLS ?
+                         "cells" : "metres", tp.ttc_grid);
+    if (tp.obst) append_launch_record(" obst=%d", tp.obst->k.K);
+    append_launch_record(" lidar=%u/%d", S, sim->num_agents);
     return F110_OK;
 }
 
@@ -2253,12 +2582,12 @@ const char *f110_last_cuda_error(void) { return g_cuda_err; }
 // at all), then k_dynamics, the planned march and the tail, with an event between them when the caller profiles.
 static int step_impl(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                      const double *actions, cudaStream_t st, cudaEvent_t *ev /* NULL or [4] */, const TailOpts *tail = nullptr,
-                     const f110_obstacles *obst = nullptr) {
+                     const f110_obstacles *obst = nullptr, const f110_lidar *lidar = nullptr) {
     int rc;
     g_launch_rec[0] = '\0';
     TickPlan tp;
     ObstPlan ob;
-    if ((rc = plan_tick(sim, map, tables, beams, actions, &tp))) return rc;
+    if ((rc = plan_tick(sim, map, tables, beams, actions, &tp, lidar))) return rc;
     if (obst) {
         if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
         tp.obst = &ob;
@@ -2276,7 +2605,11 @@ int f110_step_ex(const f110_sim *sim, const f110_map *map, const f110_march_tabl
 }
 int f110_step_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                    const double *actions, const f110_obstacles *obst, void *stream) {
-    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, nullptr, obst);
+    return f110_step_lidar(sim, map, tables, beams, actions, obst, nullptr, stream);
+}
+int f110_step_lidar(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                    const double *actions, const f110_obstacles *obst, const f110_lidar *lidar, void *stream) {
+    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, nullptr, obst, lidar);
 }
 
 int f110_step_profile(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
@@ -2419,10 +2752,15 @@ int f110_tick_ex(const f110_sim *sim, const f110_map *map, const f110_march_tabl
 int f110_tick_obst(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                    const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
                    uint64_t seed, const f110_obstacles *obst, void *stream) {
+    return f110_tick_lidar(sim, map, tables, beams, actions, env_level, start_poses, num_start, pose_gap, seed, obst, nullptr, stream);
+}
+int f110_tick_lidar(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                    const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                    uint64_t seed, const f110_obstacles *obst, const f110_lidar *lidar, void *stream) {
     int rc;
     TailOpts t;
     if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
-    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, &t, obst);
+    return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, &t, obst, lidar);
 }
 
 int f110_tick_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
@@ -2436,20 +2774,33 @@ int f110_tick_repeat_ticks_obst(const f110_sim *sim, const f110_map *map, const 
                                 const double *actions, int32_t repeat, int32_t first_tick, int32_t num_ticks, const f110_repeat *rep,
                                 int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
                                 const f110_obstacles *obst, void *stream) {
+    return f110_tick_repeat_ticks_lidar(sim, map, tables, beams, actions, repeat, first_tick, num_ticks, rep, env_level, start_poses,
+                                        num_start, pose_gap, seed, obst, nullptr, stream);
+}
+int f110_tick_repeat_ticks_lidar(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables,
+                                 const f110_beams *beams, const double *actions, int32_t repeat, int32_t first_tick,
+                                 int32_t num_ticks, const f110_repeat *rep, int32_t env_level, const double *start_poses,
+                                 int32_t num_start, int32_t pose_gap, uint64_t seed, const f110_obstacles *obst,
+                                 const f110_lidar *lidar, void *stream) {
     int rc;
     TailOpts t;
     RepeatPlan rp;
+    TickPlan last;           // the last tick of the call: the plain tick's plan, with the lidar mask
     ObstPlan ob;
     cudaStream_t st = (cudaStream_t)stream;
     if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
+    if ((rc = check_lidar(sim, lidar))) return rc;
     if (repeat < 1 || repeat > F110_MAX_REPEAT || first_tick < 0 || num_ticks < 1 || first_tick > repeat - num_ticks) return F110_ERR_INVALID;
     if (!rep || !rep->list || !rep->list_count) return F110_ERR_INVALID;
     if ((rep->done_any || rep->done_tick) && !env_level) return F110_ERR_INVALID;     // done is computed by the env-level part
     g_launch_rec[0] = '\0';
     if ((rc = plan_repeat(sim, map, tables, beams, actions, repeat, &rp))) return rc;
+    const bool masked = lidar && lidar->mask != F110_LIDAR_ALL;
+    if (masked && (rc = plan_tick(sim, map, tables, beams, actions, &last, lidar))) return rc;
     if (obst) {
         if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
         rp.tick.obst = &ob;
+        last.obst = &ob;
     }
 
     if (first_tick == 0) CUDA_TRY(cudaMemsetAsync(rep->list_count, 0, sizeof(uint32_t) * (size_t)repeat, st));
@@ -2459,7 +2810,8 @@ int f110_tick_repeat_ticks_obst(const f110_sim *sim, const f110_map *map, const 
             if ((rc = launch_ttc_tick(sim, map, beams, actions, rp, rep, tick, t, st))) return rc;
             continue;
         }
-        if ((rc = launch_tick(sim, map, tables, beams, actions, rp.tick, st, nullptr, &t))) return rc;
+        if ((rc = launch_tick(sim, map, tables, beams, actions, (masked && tick == repeat - 1) ? last : rp.tick, st, nullptr, &t)))
+            return rc;
         if (track_done) {
             RepeatDone rd;
             rd.done_any = rep->done_any; rd.done_tick = rep->done_tick; rd.tick = tick;

@@ -7,7 +7,8 @@
 // cannot fire.  Every beam's range is min(d0 + sum of non-negative steps, max_range) >= min(d0, max_range), so
 //     d0 > thr  and  max_range > thr   =>   no beam of the agent can fire: wall_flag stays 0 and nothing is marched.
 // k_ttc_select   thread per agent: lists the agents for which that is NOT true (written that way round, a NaN lists the
-//                agent) and every agent k_dynamics marked absurd; one global atomic per block.
+//                agent) and every agent k_dynamics marked absurd; one global atomic per block.  On a tick with a lidar mask
+//                (f110_lidar) only the sensorless agents are candidates: the others are in the tick's full march.
 // k_march_ttc    fixed grid, a warp per 32-beam item of a listed agent: the beam's range exactly as the tick's kernel of the
 //                map kind computes it -- cell units (k_march_lean<CELLS>, k_march_lean_het<CELLS>), metres (k_march_lean,
 //                k_march_lean_het, k_march_lean_het_res) or the rotated frame (k_march_lean_rot); the layer's geometry comes
@@ -34,6 +35,8 @@ struct TtcSelectK {
     double d0_scale;                        // metres per unit of the record's first lookup (resolution on cell-unit tables, else 1)
     double max_range;
     unsigned agents;
+    uint32_t skip;                          // lidar mask of a masked tick (f110_lidar): agents of these slots are marched in full,
+    unsigned num_agents;                    // not listed; 0 on the intermediate ticks of f110_tick_repeat
 };
 
 __global__ void __launch_bounds__(F110_TTC_SELECT_THREADS) k_ttc_select(const TtcSelectK p) {
@@ -46,7 +49,7 @@ __global__ void __launch_bounds__(F110_TTC_SELECT_THREADS) k_ttc_select(const Tt
         const double2 r1 = __ldg(p.rec + 4 * (size_t)a + 1), r2 = __ldg(p.rec + 4 * (size_t)a + 2);
         const bool absurd = (unsigned long long)__double_as_longlong(r1.y) == ~0ull;
         const bool clear = r1.x * p.d0_scale > r2.x && p.max_range > r2.x;      // false for a NaN on either side
-        listed = absurd || !clear;
+        listed = (absurd || !clear) && !(p.skip && ((p.skip >> (a % p.num_agents)) & 1u));
     }
     const unsigned vote = __ballot_sync(0xffffffffu, listed);
     unsigned wbase = 0u;

@@ -17,6 +17,7 @@ struct ObstK {
     const uint8_t *active;       // [N][K]
     int32_t *hit;                // [N*A] or NULL: the highest slot the agent touches, -1 = none
     int K;
+    uint32_t lidar;              // k_obstacles<true, true>: the lidar mask (f110_lidar); only those slots' scans are clipped
 };
 
 // the respawn draw (f110_obstacles.candidates / cand_offsets / count_* / clearance / seed), by value
@@ -57,8 +58,9 @@ __device__ __forceinline__ void obst_cast_beams(float *scan, const BeamView &bv,
     }
 }
 
-// SCAN = false: the contact part alone (the intermediate ticks of f110_tick_repeat, whose scans nobody reads)
-template <bool SCAN>
+// SCAN = false: the contact part alone (the intermediate ticks of f110_tick_repeat, whose scans nobody reads).  LIDAR: a tick
+// with a lidar mask, where the scan of an agent whose slot has no lidar does not exist and is not touched.
+template <bool SCAN, bool LIDAR = false>
 __global__ void __launch_bounds__(128) k_obstacles(f110_sim s, BeamView bv, ObstK o, double max_scan_range) {
     const int a = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -96,6 +98,7 @@ __global__ void __launch_bounds__(128) k_obstacles(f110_sim s, BeamView bv, Obst
         if (o.hit) o.hit[a] = hk;
     }
     if (!SCAN) return;
+    if (LIDAR && !((o.lidar >> (a - env * A)) & 1u)) return;
 
     // the scan, clipped against every box as against an opponent; check_ttc has zeroed the yaw of an agent whose iTTC fired
     const int hit = s.wall_flag[a];

@@ -31,6 +31,9 @@ obstacles={'candidates': (C, 5) table or one per map, 'count': (lo, hi), 'cleara
 Simulator.set_obstacles / set_obstacle_draw with hi slots per env): static box obstacles, redrawn on the device for every env by
 reset() after it places the agents and for the masked envs by reset_envs(); obs['obstacles'] (N, K, 5) and
 obs['obstacle_active'] (N, K) are views of the device buffers, and local_map / rgb_array draw the boxes (class 5).
+lidar=[True, False, ...] (batched mode only; Simulator.set_lidar): which agent slots have a lidar.  A sensorless agent (a
+scripted opponent, a policy on state or local_map observations) is simulated as before, and its row of obs['scans'] is NaN.
+Its scan is skipped only without scan noise (scan_noise_std=0.0): with the default 0.01 every scan is still computed.
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
@@ -74,6 +77,13 @@ class F110Env(object):
         if isinstance(self.map_path, (list, tuple)) and not self.batched:
             raise ValueError('a list of maps needs the batched mode (num_envs)')
         self._obstacles = self._obstacle_settings(kwargs.get('obstacles', None), self.batched)
+        lidar = kwargs.get('lidar', None)
+        if lidar is not None:
+            if not self.batched:
+                raise ValueError('lidar= needs the batched mode (num_envs): single-env mode runs on Simulator.step_host')
+            lidar = [bool(v) for v in lidar]
+            if len(lidar) != self.num_agents:
+                raise ValueError('lidar needs one bool per agent (%d), got %d' % (self.num_agents, len(lidar)))
         self.start_thresh = 0.5
         self.sim = Simulator(self.params, self.num_agents, self.seed, time_step=self.timestep,
                              ego_idx=self.ego_idx, integrator=self.integrator, lidar_dist=self.lidar_dist,
@@ -94,6 +104,8 @@ class F110Env(object):
             raise ValueError('action_repeat must be an int in [1, 64], got %r' % (self.action_repeat,))
         self.action_repeat = int(self.action_repeat)
         self._set_map(self.map_path, self.map_ext)
+        if lidar is not None:
+            self.sim.set_lidar(lidar)
         if self._obstacles is not None:
             cand, count, clearance, seed = self._obstacles
             self.sim.set_obstacles(np.zeros((count[1], 5)), np.zeros(count[1], bool))

@@ -414,6 +414,10 @@ class Simulator(object):
         self._obst = None
         self.obstacle_boxes = self.obstacle_active = self.obstacle_hit = None
         self._obst_keep = ()
+        # agents without a lidar (C ABI f110_lidar), set by set_lidar; None: every slot has one
+        self._lidar = None
+        self._lidar_slots = (True,) * A
+        self.lidar_list = self.lidar_list_count = self.lidar_listed = None
 
     # ------------------------------------------------------------------ configuration
     def set_map(self, map_path, map_ext, edt='scipy'):
@@ -545,8 +549,9 @@ class Simulator(object):
     def step(self, control_inputs):
         """Simulator.step (base_classes.py:553-612). control_inputs (N,A,2) = (steer, speed)."""
         a = self._actions_tensor(control_inputs)
-        nat.check(nat.lib().f110_step_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                           C.byref(self.beams.c), nat.ptr(a), self._obst_ref(), _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_step_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                            C.byref(self.beams.c), nat.ptr(a), self._obst_ref(), self._lidar_ref(),
+                                            _stream_ptr(self.device)))
         return self.observations()
 
     def env_post_step(self):
@@ -586,10 +591,61 @@ class Simulator(object):
         results as step(); env_post_step(); autoreset()."""
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
-        nat.check(nat.lib().f110_tick_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                           C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
-                                           int(seed), self._obst_ref(), _stream_ptr(self.device)))
+        nat.check(nat.lib().f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                            C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
+                                            int(seed), self._obst_ref(), self._lidar_ref(), _stream_ptr(self.device)))
         return self.observations()
+
+    # ------------------------------------------------------------------ agents without a lidar
+    def set_lidar(self, slots):
+        """Which agent slots have a lidar (C ABI f110_lidar): a length-A sequence of bools, the same for every env, or None for
+        all.  A sensorless agent is simulated exactly as before -- dynamics, the iTTC wall check on its wall-only scan, collisions,
+        lap logic, done, auto-reset, obstacle contact -- and the other agents still see its body; only its own scan is not
+        computed.  Its row of `scans` is filled with NaN here, once, and no tick writes it while the short path runs (no scan
+        noise, a lean ray march, beams.side_max below max_range, at most 32 agents per env); on any other configuration the mask
+        is ignored and every scan is computed as without it.  step, tick, tick_repeat (its last tick) and capture_graph use the
+        mask; the host-buffer paths and step_profile raise ValueError while a slot is sensorless.  A slot that gets its lidar
+        back has its scan from the next tick on.  Drops a captured graph.  ValueError for a wrong length, or for more than 32
+        agents with a False entry."""
+        A, N = self.num_agents, self.num_envs
+        new = (True,) * A if slots is None else tuple(bool(v) for v in slots)
+        if len(new) != A:
+            raise ValueError('lidar needs one bool per agent slot (%d), got %d' % (A, len(new)))
+        if not all(new) and A > 32:
+            raise ValueError('a lidar mask covers at most 32 agent slots, this simulator has %d' % A)
+        old = self._lidar_slots
+        self._lidar_slots = new
+        self._graph = None
+        if all(new):
+            self._lidar = None
+        else:
+            if self.lidar_list is None:
+                dev = self.device
+                self.lidar_list = torch.zeros((N * A,), dtype=torch.int32, device=dev)
+                self.lidar_list_count = torch.zeros((1,), dtype=torch.int32, device=dev)
+                self.lidar_listed = torch.zeros((1,), dtype=torch.int64, device=dev)
+            mask = sum(1 << i for i, v in enumerate(new) if v)
+            self._lidar = nat.F110Lidar(mask, nat.ptr(self.lidar_list), nat.ptr(self.lidar_list_count),
+                                        nat.ptr(self.lidar_listed))
+            off = [i for i, v in enumerate(new) if not v and old[i]]
+            if off:     # so that a stale row cannot pass for a scan
+                self.scans.view(N, A, self.num_beams)[:, off] = float('nan')
+        back = [i for i, v in enumerate(new) if v and not old[i]]
+        if back and self.march_cost is not None:
+            # no lookup history while the slot was sensorless: its items are queued as very heavy, as after a reset
+            self.march_cost.view(N, A, 256)[:, back] = -1
+
+    @property
+    def lidar(self):
+        """Which agent slots have a lidar (set_lidar): a tuple of A bools."""
+        return self._lidar_slots
+
+    def _lidar_ref(self):
+        return None if self._lidar is None else C.byref(self._lidar)
+
+    def _no_lidar_mask(self, who):
+        if self._lidar is not None:
+            raise ValueError('%s computes every scan; call set_lidar(None) first or use step / tick' % who)
 
     # ------------------------------------------------------------------ static box obstacles
     def _obst_ref(self):
@@ -709,10 +765,10 @@ class Simulator(object):
         """Enqueue one f110_tick_repeat call; progress: the tracker is updated after every tick of the call (the same ticks,
         issued one by one) and track_delta_sum gets the sum of the call's deltas."""
         def ticks(first, count):
-            nat.check(L.f110_tick_repeat_ticks_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                                    C.byref(self.beams.c), nat.ptr(actions), K, first, count, C.byref(call),
-                                                    1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(seed),
-                                                    self._obst_ref(), _stream_ptr(self.device)))
+            nat.check(L.f110_tick_repeat_ticks_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                                     C.byref(self.beams.c), nat.ptr(actions), K, first, count, C.byref(call),
+                                                     1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(seed),
+                                                     self._obst_ref(), self._lidar_ref(), _stream_ptr(self.device)))
         if not progress:
             ticks(0, K)
             return
@@ -940,7 +996,8 @@ class Simulator(object):
                  'start_ys', 'start_thetas', 'start_rot', 'done', 'checkpoint_done', 'tick_counter', 'march_cost',
                  'march_order', 'march_count', 'march_rec', 'track_seg', 'track_s', 'track_d', 'track_heading_error',
                  'track_progress', 'track_delta', 'done_any', 'done_tick', 'repeat_list', 'repeat_list_count',
-                 'marched_agents', 'track_delta_sum', 'obstacle_boxes', 'obstacle_active', 'obstacle_hit')
+                 'marched_agents', 'track_delta_sum', 'obstacle_boxes', 'obstacle_active', 'obstacle_hit', 'lidar_list',
+                 'lidar_list_count', 'lidar_listed')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
 
@@ -948,9 +1005,10 @@ class Simulator(object):
             if K > 1:
                 self._issue_repeat(L, actions, K, call, env_level, table, num_start, pose_gap, autoreset_seed, progress)
                 return
-            nat.check(L.f110_tick_obst(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                       C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
-                                       pose_gap, int(autoreset_seed), self._obst_ref(), _stream_ptr(self.device)))
+            nat.check(L.f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                        C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
+                                        pose_gap, int(autoreset_seed), self._obst_ref(), self._lidar_ref(),
+                                        _stream_ptr(self.device)))
             if progress:
                 self._launch_progress(L)
         side = torch.cuda.Stream(self.device)
@@ -968,7 +1026,8 @@ class Simulator(object):
         self._graph = g
         self._graph_keep = (actions, table) + ((self.centerlines, self._progress_views) if progress else ()) + \
             ((call,) if K > 1 else ()) + ((self._obst, self.obstacle_boxes, self.obstacle_active, self.obstacle_hit) +
-                                          self._obst_keep if self._obst is not None else ())
+                                          self._obst_keep if self._obst is not None else ()) + \
+            ((self._lidar, self.lidar_list, self.lidar_list_count, self.lidar_listed) if self._lidar is not None else ())
         return g
 
     def replay(self):
@@ -977,6 +1036,7 @@ class Simulator(object):
     def make_host_io(self, with_scans=True, packed_scans=False):
         """Pinned host buffers for step_host() / step_host_async().  packed_scans=True (async path only): the scan block
         crosses PCIe as 24-bit fixed point (io['scans_u24'] uint8 [NA, B, 3]; decode with unpack_scans_u24) instead of fp32."""
+        self._no_lidar_mask('make_host_io')
         N, A, B = self.num_envs, self.num_agents, self.num_beams
         NA = N * A
         if packed_scans:
@@ -1004,6 +1064,7 @@ class Simulator(object):
         """One tick through HOST buffers (C ABI f110_step_host): H2D actions, step, env_post_step,
         D2H observation, stream sync.  io from make_host_io(); fill io['actions'] first.  ValueError with obstacles set."""
         self._no_obstacles('step_host')
+        self._no_lidar_mask('step_host')
         nat.check(nat.lib().f110_step_host(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c),
                                            nat.ptr(io['actions']), nat.ptr(self._actions_dev),
                                            C.byref(io['_struct']), _stream_ptr(self.device)))
@@ -1014,6 +1075,7 @@ class Simulator(object):
         step_host_async(); one shared copy stream.  packed_scans=True: ValueError for a map whose max_range plus 8 sigma of
         the scan noise reaches 32 m, where the 24-bit block clamps (step_host_async checks again once the map or the noise
         changed)."""
+        self._no_lidar_mask('make_host_pipeline')
         N, A, B = self.num_envs, self.num_agents, self.num_beams
         NA = N * A
         dev = self.device
@@ -1062,6 +1124,7 @@ class Simulator(object):
         (before anything is enqueued) when the map or the noise changed since the last check and now reaches 32 m.  ValueError
         with obstacles set."""
         self._no_obstacles('step_host_async')
+        self._no_lidar_mask('step_host_async')
         if io['scans_u24'] is not None:
             checked = io.get('_packed_checked')
             if checked is None or checked[0] is not self._map_struct or checked[1] != self.c.noise_std:
@@ -1082,6 +1145,7 @@ class Simulator(object):
         """One tick with CUDA events around each kernel -> (dynamics_ms, raymarch_ms, finalize_ms).  ValueError with obstacles
         set."""
         self._no_obstacles('step_profile')
+        self._no_lidar_mask('step_profile')
         a = self._actions_tensor(control_inputs)
         ms = (C.c_float * 3)()
         nat.check(nat.lib().f110_step_profile_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),

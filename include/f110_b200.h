@@ -346,6 +346,42 @@ int f110_autoreset_obst(const f110_sim *sim, const double *start_poses, int32_t 
  * draws its start poses with.  F110_ERR_INVALID also without candidates and with more than 32 agents per env. */
 int f110_obstacles_respawn(const f110_sim *sim, const f110_obstacles *obst, const uint8_t *env_mask, uint64_t tick, void *stream);
 
+/* ---- agents without a lidar (batch extension; csrc/march_ttc.cuh) ---- */
+/* A lidar mask says which agent slots have a lidar: bit i covers slot i in every env.  A sensorless agent is simulated exactly
+ * as one with a lidar -- dynamics, steer FIFO, the iTTC wall check on its wall-only scan (state[3:] zeroed on a hit), GJK,
+ * collisions / collision_idx, lap logic, done, auto-reset and obstacle contact -- and the other agents still see its body in
+ * their scans; only its own scan is never computed.
+ * Short path: when the tick's ray march is a lean kernel, the scan noise is off, beams->side_max is known and below max_range,
+ * dt_min_positive > eps and A <= 32 (the conditions of the short path of f110_tick_repeat), the march queue holds the items of
+ * the slots that have a lidar only, the sensorless agents a wall could stop are listed and marched for the iTTC flag alone, and
+ * no kernel writes a sensorless agent's scan row.  Every buffer of f110_sim then equals, bit for bit, what the call without a
+ * mask leaves, except the scan rows of sensorless agents, march_cost / march_order / march_count and *lookup_counter; the scans
+ * of the agents that have a lidar are bit-identical, opponent ray-cast and obstacle clip included.
+ * Full path: otherwise the mask is ignored and the call equals the call without it, scans included. */
+#define F110_LIDAR_ALL 0xFFFFFFFFu
+typedef struct {
+    uint32_t mask;                  /* bit i: slot i has a lidar; F110_LIDAR_ALL = every slot (any A) */
+    uint32_t *list;                 /* [N*A] device scratch: sensorless agents listed for the iTTC-only march */
+    uint32_t *list_count;           /* [1] device scratch, zeroed by the call on `stream` */
+    unsigned long long *listed;     /* [1] or NULL: += sensorless agents listed (measurement) */
+} f110_lidar;
+
+/* The _obst calls with a lidar mask.  lidar == NULL or mask == F110_LIDAR_ALL is exactly the _obst call.  F110_ERR_INVALID
+ * before anything is enqueued for any other mask with more than 32 agents per env, a bit set at or above num_agents, and NULL
+ * list or list_count with a mask other than F110_LIDAR_ALL (on either path).  f110_tick_repeat_ticks_lidar applies the mask
+ * to the last tick of the call; the ticks before it run as in f110_tick_repeat_ticks_obst.  No allocation, no host
+ * synchronisation: capturable in a CUDA graph. */
+int f110_step_lidar(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                    const double *actions, const f110_obstacles *obst, const f110_lidar *lidar, void *stream);
+int f110_tick_lidar(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                    const double *actions, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                    uint64_t seed, const f110_obstacles *obst, const f110_lidar *lidar, void *stream);
+int f110_tick_repeat_ticks_lidar(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables,
+                                 const f110_beams *beams, const double *actions, int32_t repeat, int32_t first_tick,
+                                 int32_t num_ticks, const f110_repeat *rep, int32_t env_level, const double *start_poses,
+                                 int32_t num_start, int32_t pose_gap, uint64_t seed, const f110_obstacles *obst,
+                                 const f110_lidar *lidar, void *stream);
+
 /* Same tick through HOST buffers: copies actions H2D, runs f110_step (+ f110_env_post_step when the
  * lap arrays are bound), copies the observation D2H and synchronises the stream.
  * Any output pointer may be NULL to skip that copy.  Host buffers should be pinned. */
