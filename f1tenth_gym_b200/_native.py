@@ -98,6 +98,13 @@ class F110Lidar(C.Structure):
 
 LIDAR_ALL = 0xFFFFFFFF
 
+
+class F110Episodes(C.Structure):
+    """include/f110_episodes.h f110_episodes."""
+    _fields_ = [('max_ticks', C.c_int32), ('ticks', _dp), ('terminated', _dp), ('truncated', _dp), ('length', _dp),
+                ('final_state', _dp), ('final_scans', _dp), ('final_collisions', _dp), ('final_collision_idx', _dp),
+                ('final_lap_times', _dp), ('final_lap_counts', _dp), ('list', _dp), ('list_count', _dp), ('track_seg', _dp)]
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol declared
 # in include/f110_b200.h is exported.
 _P = C.POINTER
@@ -172,6 +179,12 @@ SIGNATURES = {
 }
 
 # measurement / test aids exported by the library but not part of the public header
+# the entry points of include/f110_episodes.h (episode mode), bound like SIGNATURES
+EPISODE_SIGNATURES = {
+    'f110_tick_episodes': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, _dp, C.c_int32, C.c_int32,
+                                     C.c_uint64, _P(F110Obstacles), _P(F110Lidar), _P(F110Episodes), _dp]),
+}
+
 DEBUG_SIGNATURES = {
     'f110_debug_set_variant': (None, [C.c_int]),
     'f110_debug_set_chunk': (None, [C.c_int]),
@@ -211,7 +224,7 @@ def lib():
         L = C.CDLL(LIB_PATH)
     except OSError as e:
         raise NativeLibraryError('f1tenth_gym_b200: cannot load %s: %s' % (LIB_PATH, e))
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in list(SIGNATURES.items()) + list(EPISODE_SIGNATURES.items()):
         try:
             f = getattr(L, name)
         except AttributeError:

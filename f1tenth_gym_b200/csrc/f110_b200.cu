@@ -28,6 +28,7 @@
 #include <type_traits>
 
 #include "../../include/f110_b200.h"
+#include "../../include/f110_episodes.h"
 #include "collision.cuh"
 #include "dynamics.cuh"
 #include "lidar.cuh"
@@ -1146,6 +1147,7 @@ __global__ void __launch_bounds__(32 * F110_LIDAR_CAST_WARPS) k_lidar_cast(f110_
 
 }  // namespace f110
 #include "obstacles.cuh"     // k_obstacles, k_env_tail_obst: built on the tail's device functions above
+#include "episodes.cuh"      // the restart of ended episodes: built on the same functions and on obstacles.cuh's
 namespace f110 {
 
 // f110_track_progress_sum: the deltas of the ticks of one policy step, summed in tick order
@@ -2513,6 +2515,39 @@ static int launch_lidar_tick(const f110_sim *sim, const f110_map *map, const f11
     return F110_OK;
 }
 
+// ---- episodes (csrc/episodes.cuh): the plain tick, then the end decision and the restart of the ended envs
+// The restart march reuses k_march_ttc's beam arithmetic, which covers the lean march families only.
+static bool episode_march_ok(const MarchPlan &m) {
+    return m.lean && (m.family == MarchFamily::LEAN || m.family == MarchFamily::LEAN_BRICK || m.family == MarchFamily::LEAN_HET ||
+                      m.family == MarchFamily::LEAN_HET_RES || m.family == MarchFamily::LEAN_ROT);
+}
+template <int UNITS>
+static int restart_grid(bool count, unsigned *grid) {
+    static int per_sm[2] = {0, 0};
+    int &n = per_sm[count ? 1 : 0];
+    if (n <= 0) {
+        if (count) CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_restart_march<UNITS, true>, F110_TTC_THREADS, 0));
+        else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_restart_march<UNITS, false>, F110_TTC_THREADS, 0));
+        if (n <= 0) return F110_ERR_INVALID;
+    }
+    *grid = (unsigned)n * (unsigned)num_sms();
+    return F110_OK;
+}
+template <int UNITS>
+static void launch_restart_march_t(const TtcK &q, const RestartK &r, bool count, unsigned grid, cudaStream_t st) {
+    if (count) k_restart_march<UNITS, true><<<grid, F110_TTC_THREADS, 0, st>>>(q, r);
+    else k_restart_march<UNITS, false><<<grid, F110_TTC_THREADS, 0, st>>>(q, r);
+}
+static int check_episodes(const f110_sim *sim, const f110_episodes *ep, const double *start_poses) {
+    if (!ep || !start_poses) return F110_ERR_INVALID;
+    if (!ep->ticks || !ep->terminated || !ep->truncated || !ep->length || !ep->final_state || !ep->final_scans ||
+        !ep->final_collisions || !ep->final_collision_idx || !ep->final_lap_times || !ep->final_lap_counts || !ep->list ||
+        !ep->list_count)
+        return F110_ERR_INVALID;
+    if (ep->max_ticks < 0 || sim->num_agents > 32) return F110_ERR_INVALID;
+    return F110_OK;
+}
+
 }  // namespace f110
 
 using namespace f110;
@@ -2761,6 +2796,83 @@ int f110_tick_lidar(const f110_sim *sim, const f110_map *map, const f110_march_t
     TailOpts t;
     if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
     return step_impl(sim, map, tables, beams, actions, (cudaStream_t)stream, nullptr, &t, obst, lidar);
+}
+
+int f110_tick_episodes(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                       const double *actions, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
+                       const f110_obstacles *obst, const f110_lidar *lidar, const f110_episodes *ep, void *stream) {
+    int rc;
+    TailOpts t;
+    TickPlan tp;
+    ObstPlan ob;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = tick_tail_opts(sim, map, 1, start_poses, num_start, pose_gap, seed, &t))) return rc;
+    if ((rc = check_episodes(sim, ep, start_poses))) return rc;
+    const AutoResetArgs ar = t.ar;
+    t.ar.start_poses = nullptr;          // the plain tick runs without the auto-reset; k_episode_end restarts the ended envs
+    g_launch_rec[0] = '\0';
+    if ((rc = plan_tick(sim, map, tables, beams, actions, &tp, lidar))) return rc;
+    if (!episode_march_ok(tp.march)) return F110_ERR_INVALID;
+    if (obst) {
+        if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
+        tp.obst = &ob;
+    }
+    const int units = tp.march.rot ? F110_SCAN_UNITS_ROT : tp.march.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+    unsigned grid = 0u;
+    if ((rc = units == F110_SCAN_UNITS_ROT ? restart_grid<F110_SCAN_UNITS_ROT>(tp.march.count, &grid)
+            : units == F110_SCAN_UNITS_CELLS ? restart_grid<F110_SCAN_UNITS_CELLS>(tp.march.count, &grid)
+                                             : restart_grid<F110_SCAN_UNITS_METRES>(tp.march.count, &grid)))
+        return rc;
+
+    if ((rc = launch_tick(sim, map, tables, beams, actions, tp, st, nullptr, &t))) return rc;
+    const int N = sim->num_envs, A = sim->num_agents, NA = N * A;
+    const uint32_t all = A == 32 ? 0xFFFFFFFFu : (1u << A) - 1u;
+    // the slots whose scans exist: the mask on the short path, every slot when the tick ignores it (or has none)
+    const uint32_t scan_slots = tp.lidar ? tp.lidar->mask : all;
+    const uint32_t final_slots = (lidar && lidar->mask != F110_LIDAR_ALL) ? (lidar->mask & all) : all;
+    EpisodeK k;
+    k.ticks = ep->ticks; k.length = ep->length; k.terminated = ep->terminated; k.truncated = ep->truncated;
+    k.final_state = ep->final_state; k.final_collisions = ep->final_collisions; k.final_lap_times = ep->final_lap_times;
+    k.final_lap_counts = ep->final_lap_counts; k.final_collision_idx = ep->final_collision_idx;
+    k.list = ep->list; k.count = ep->list_count; k.track_seg = ep->track_seg; k.max_ticks = ep->max_ticks;
+    ObstDraw no_draw;
+    memset(&no_draw, 0, sizeof(no_draw));
+    CUDA_TRY(cudaMemsetAsync(ep->list_count, 0, sizeof(uint32_t), st));
+    k_episode_end<<<(N + 127) / 128, 128, 0, st>>>(*sim, ar, k, obst ? ob.d : no_draw);
+    LAUNCH_CHECK("k_episode_end");
+    k_episode_dyn<<<(NA + 127) / 128, 128, 0, st>>>(*sim, beams->fov, (double)map->theta_dis,
+                                                    fill_first_lookup(sim, map, beams, tp.geom, tp.march), ep->list, ep->list_count);
+    LAUNCH_CHECK("k_episode_dyn");
+    RestartK r;
+    r.list = ep->list; r.count = ep->list_count; r.scans = sim->scans; r.final_scans = ep->final_scans;
+    r.tick_counter = sim->tick_counter; r.noise_std = sim->noise_std; r.noise_seed = sim->noise_seed;
+    r.lidar = scan_slots; r.final_slots = final_slots;
+    const TtcK q = fill_ttc_k(sim, map, beams, tp, ep->list, ep->list_count);
+    if (units == F110_SCAN_UNITS_ROT) launch_restart_march_t<F110_SCAN_UNITS_ROT>(q, r, tp.march.count, grid, st);
+    else if (units == F110_SCAN_UNITS_CELLS) launch_restart_march_t<F110_SCAN_UNITS_CELLS>(q, r, tp.march.count, grid, st);
+    else launch_restart_march_t<F110_SCAN_UNITS_METRES>(q, r, tp.march.count, grid, st);
+    LAUNCH_CHECK("k_restart_march");
+    const BeamView bv = make_view(beams);
+    const double max_scan = max_scan_range(sim, map);
+    const unsigned slots = (unsigned)__builtin_popcount(scan_slots);
+    if (A > 1 && slots) {
+        const LidarOrder lo = {scan_slots, slots};
+        k_episode_cast<<<(unsigned)(((unsigned long long)N * slots + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS),
+                         32 * F110_LIDAR_CAST_WARPS, 0, st>>>(*sim, bv, lo, ep->list, ep->list_count, max_scan);
+        LAUNCH_CHECK("k_episode_cast");
+    }
+    k_episode_tail<<<(N + 127) / 128, 128, 0, st>>>(*sim, ep->list, ep->list_count);
+    LAUNCH_CHECK("k_episode_tail");
+    if (obst) {
+        ObstK o = ob.k;
+        o.lidar = scan_slots;
+        k_episode_obstacles<<<(unsigned)(((long long)NA * 32 + 127) / 128), 128, 0, st>>>(*sim, bv, o, max_scan, ep->list,
+                                                                                          ep->list_count);
+        LAUNCH_CHECK("k_episode_obstacles");
+    }
+    append_launch_record(" episodes restart=k_episode_end+k_episode_dyn+k_restart_march%s+k_episode_tail%s",
+                         (A > 1 && slots) ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "");
+    return F110_OK;
 }
 
 int f110_tick_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,

@@ -60,11 +60,10 @@ __device__ __forceinline__ void obst_cast_beams(float *scan, const BeamView &bv,
 
 // SCAN = false: the contact part alone (the intermediate ticks of f110_tick_repeat, whose scans nobody reads).  LIDAR: a tick
 // with a lidar mask, where the scan of an agent whose slot has no lidar does not exist and is not touched.
-template <bool SCAN, bool LIDAR = false>
-__global__ void __launch_bounds__(128) k_obstacles(f110_sim s, BeamView bv, ObstK o, double max_scan_range) {
-    const int a = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (a >= s.num_envs * s.num_agents) return;
+// obstacles_agent: the work of agent a's warp, shared with the restarted envs' instance (k_episode_obstacles, episodes.cuh)
+template <bool SCAN, bool LIDAR>
+__device__ __forceinline__ void obstacles_agent(const f110_sim &s, const BeamView &bv, const ObstK &o, double max_scan_range,
+                                                int a, int lane) {
     const int A = s.num_agents, env = a / A;
     const double *pa = s.agent_poses + 5 * (size_t)a;
     const double *boxes = o.boxes + (size_t)env * o.K * 5;
@@ -143,6 +142,14 @@ __global__ void __launch_bounds__(128) k_obstacles(f110_sim s, BeamView bv, Obst
         }
         __syncwarp();
     }
+}
+
+template <bool SCAN, bool LIDAR = false>
+__global__ void __launch_bounds__(128) k_obstacles(f110_sim s, BeamView bv, ObstK o, double max_scan_range) {
+    const int a = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (a >= s.num_envs * s.num_agents) return;
+    obstacles_agent<SCAN, LIDAR>(s, bv, o, max_scan_range, a, lane);
 }
 
 // u in [0, 1) from the top 53 bits of a hash, as the auto-reset's start-pose draw

@@ -34,6 +34,13 @@ obs['obstacle_active'] (N, K) are views of the device buffers, and local_map / r
 lidar=[True, False, ...] (batched mode only; Simulator.set_lidar): which agent slots have a lidar.  A sensorless agent (a
 scripted opponent, a policy on state or local_map observations) is simulated as before, and its row of obs['scans'] is NaN.
 Its scan is skipped only without scan noise (scan_noise_std=0.0): with the default 0.01 every scan is still computed.
+autoreset={'poses': (K, 3) start table or one per map, 'max_episode_steps': T, 'seed': s, 'pose_gap': g} (batched mode only,
+action_repeat 1; Simulator.set_episodes): step() ends the episode of every env that is done or has run T steps (None or 0: no
+limit) and restarts it on the device as reset() would: a start pose drawn from the table, then one zero-action tick, whose
+observation obs holds for that env.  done = terminated | truncated; info adds 'terminated', 'truncated', 'episode_length' and
+'final_observation' (the ended episode's last observation: state keys, scans, collisions, lap_times, lap_counts).  All are
+views of device buffers, overwritten by the next step.  local_map and the progress keys are those after the restart; with
+reward='progress' a restarted env earns 0 on that step.  reset() and reset_envs() zero the episode counters.
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
@@ -84,6 +91,8 @@ class F110Env(object):
             lidar = [bool(v) for v in lidar]
             if len(lidar) != self.num_agents:
                 raise ValueError('lidar needs one bool per agent (%d), got %d' % (self.num_agents, len(lidar)))
+        self._autoreset = self._autoreset_settings(kwargs.get('autoreset', None), self.batched,
+                                                   kwargs.get('action_repeat', 1))
         self.start_thresh = 0.5
         self.sim = Simulator(self.params, self.num_agents, self.seed, time_step=self.timestep,
                              ego_idx=self.ego_idx, integrator=self.integrator, lidar_dist=self.lidar_dist,
@@ -106,6 +115,10 @@ class F110Env(object):
         self._set_map(self.map_path, self.map_ext)
         if lidar is not None:
             self.sim.set_lidar(lidar)
+        if self._autoreset is not None:
+            self.sim.set_episodes(self._autoreset['max_episode_steps'])
+            p = self._autoreset['poses']
+            self._autoreset['poses'] = [t.to(self.sim.device) for t in p] if isinstance(p, list) else p.to(self.sim.device).contiguous()
         if self._obstacles is not None:
             cand, count, clearance, seed = self._obstacles
             self.sim.set_obstacles(np.zeros((count[1], 5)), np.zeros(count[1], bool))
@@ -142,9 +155,10 @@ class F110Env(object):
         t = t.view(self.num_envs, self.num_agents)
         return t if self.batched else t[0].cpu().numpy()
 
-    def _finish(self, obs):
+    def _finish(self, obs, episode=False):
         sim = self.sim
-        sim.env_post_step()
+        if not episode:
+            sim.env_post_step()
         N, A = self.num_envs, self.num_agents
         reward = self.timestep
         if self.batched:
@@ -162,6 +176,11 @@ class F110Env(object):
                     reward = p['delta'][:, self.ego_idx].clone()
             done = sim.done.bool()
             info = {'checkpoint_done': sim.checkpoint_done.view(N, A).bool()}
+            if episode:
+                term, trunc = obs.pop('terminated').bool(), obs.pop('truncated').bool()
+                done = term | trunc
+                info.update(terminated=term, truncated=trunc, episode_length=sim.episode_length,
+                            final_observation=sim.final_observation)
             return obs, reward, done, info
         # single-env, reference-shaped (base_classes.py:594-612): lists of per-agent values
         o = {'ego_idx': obs['ego_idx'],
@@ -214,6 +233,10 @@ class F110Env(object):
             return self._step_repeat(action)
         if not self.batched:
             return self._step_single(action)
+        if self._autoreset is not None:
+            ar = self._autoreset
+            obs = self.sim.tick(action, env_level=True, autoreset_poses=ar['poses'], pose_gap=ar['pose_gap'], seed=ar['seed'])
+            return self._finish(obs, episode=True)
         obs = self.sim.step(action)
         return self._finish(obs)
 
@@ -262,6 +285,33 @@ class F110Env(object):
         self.sim.env_reset(poses, env_mask)
         if self._obstacles is not None:
             self.sim.respawn_obstacles(env_mask)
+
+    def _autoreset_settings(self, cfg, batched, action_repeat):
+        """autoreset kwarg -> {'poses': device table or list, 'max_episode_steps', 'seed', 'pose_gap'}, or None; ValueError
+        before any device work."""
+        if cfg is None:
+            return None
+        if not batched:
+            raise ValueError('autoreset needs the batched mode (num_envs)')
+        if action_repeat != 1:
+            raise ValueError('autoreset runs with action_repeat=1 only')
+        if not isinstance(cfg, dict) or 'poses' not in cfg or set(cfg) - {'poses', 'max_episode_steps', 'seed', 'pose_gap'}:
+            raise ValueError("autoreset must be a dict with 'poses' and optionally 'max_episode_steps', 'seed', 'pose_gap', got %r"
+                             % (cfg,))
+        T = cfg.get('max_episode_steps', None)
+        T = 0 if T is None else T
+        if isinstance(T, bool) or int(T) != T or int(T) < 0:
+            raise ValueError('autoreset max_episode_steps must be None or an int >= 0, got %r' % (T,))
+        poses = cfg['poses']
+        tables = poses if isinstance(poses, (list, tuple)) else [poses]
+        for t in tables:
+            a = np.asarray(t.cpu() if torch.is_tensor(t) else t, dtype=np.float64)
+            if a.ndim != 2 or a.shape[1] != 3 or a.shape[0] < 1 or not np.all(np.isfinite(a)):
+                raise ValueError('autoreset poses must be (K, 3) finite start poses, or a list of them (one per map)')
+        to_dev = lambda t: torch.as_tensor(np.asarray(t.cpu() if torch.is_tensor(t) else t, dtype=np.float64))
+        table = [to_dev(t) for t in poses] if isinstance(poses, (list, tuple)) else to_dev(poses)
+        return {'poses': table, 'max_episode_steps': int(T), 'seed': int(cfg.get('seed', 12345)),
+                'pose_gap': int(cfg.get('pose_gap', 23))}
 
     def _obstacle_obs(self, obs):
         if self._obstacles is not None:

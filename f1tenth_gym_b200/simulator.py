@@ -418,6 +418,11 @@ class Simulator(object):
         self._lidar = None
         self._lidar_slots = (True,) * A
         self.lidar_list = self.lidar_list_count = self.lidar_listed = None
+        # episode mode (C ABI f110_episodes), set by set_episodes; None: off
+        self._episodes = None
+        self.ep_ticks = self.ep_terminated = self.ep_truncated = self.ep_length = None
+        self.final_state = self.final_scans = self.final_collisions = self.final_collision_idx = None
+        self.final_lap_times = self.final_lap_counts = self.ep_list = self.ep_list_count = None
 
     # ------------------------------------------------------------------ configuration
     def set_map(self, map_path, map_ext, edt='scipy'):
@@ -536,6 +541,11 @@ class Simulator(object):
         nat.check(L.f110_env_reset(C.byref(self.c), nat.ptr(p), mp, _stream_ptr(self.device)))
         nat.check(L.f110_reset(C.byref(self.c), nat.ptr(p), mp, _stream_ptr(self.device)))
         self._unacquire(m)
+        if self.ep_ticks is not None:       # a device-side masked fill: no host synchronisation
+            if m is None:
+                self.ep_ticks.zero_()
+            else:
+                self.ep_ticks.masked_fill_(m.bool(), 0)
 
     def _unacquire(self, mask):
         """seg = -1 (not acquired) for the agents of the masked envs (mask: (N,) uint8 device tensor, or None = all)."""
@@ -591,10 +601,107 @@ class Simulator(object):
         results as step(); env_post_step(); autoreset()."""
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
+        if self._episode_path(table, env_level):
+            self._launch_episodes(nat.lib(), a, table, n, pose_gap, seed)
+            obs = self.observations()
+            obs['terminated'], obs['truncated'] = self.ep_terminated, self.ep_truncated
+            return obs
         nat.check(nat.lib().f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
                                             C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
                                             int(seed), self._obst_ref(), self._lidar_ref(), _stream_ptr(self.device)))
         return self.observations()
+
+    # ------------------------------------------------------------------ episodes
+    def set_episodes(self, max_ticks=None):
+        """Episode mode (C ABI f110_tick_episodes, include/f110_episodes.h): tick() and capture_graph() with autoreset_poses then
+        end an env's episode when it is done (terminated: ego collision or every agent checkpoint-done) or has run max_ticks
+        ticks (truncated; None or 0: no time limit), keep its final observation in final_observation, and restart it as
+        F110Env.reset does: the auto-reset's start-pose draw, then one zero-action tick of that env alone, whose observation
+        the env then holds.  The tick that ends an episode still reports done = 1.  False turns the mode off.  Drops a
+        captured graph.  ValueError for a negative max_ticks or more than 32 agents per env."""
+        self._graph = None
+        if max_ticks is False:
+            self._episodes = None
+            self.ep_ticks = self.ep_terminated = self.ep_truncated = self.ep_length = None
+            self.final_state = self.final_scans = self.final_collisions = self.final_collision_idx = None
+            self.final_lap_times = self.final_lap_counts = self.ep_list = self.ep_list_count = None
+            return
+        T = 0 if max_ticks is None else max_ticks
+        if isinstance(T, bool) or int(T) != T or int(T) < 0 or int(T) > 0x7FFFFFFF:
+            raise ValueError('max_ticks must be None or an int >= 0, got %r' % (max_ticks,))
+        if self.num_agents > 32:
+            raise ValueError('episode mode restarts envs of at most 32 agents, this simulator has %d' % self.num_agents)
+        N, NA, dev = self.num_envs, self.num_envs * self.num_agents, self.device
+        if self._episodes is None:
+            f64 = dict(dtype=torch.float64, device=dev)
+            self.ep_ticks = torch.zeros((N,), dtype=torch.int32, device=dev)
+            self.ep_terminated = torch.zeros((N,), dtype=torch.uint8, device=dev)
+            self.ep_truncated = torch.zeros((N,), dtype=torch.uint8, device=dev)
+            self.ep_length = torch.zeros((N,), dtype=torch.int32, device=dev)
+            self.final_state = torch.zeros((7, NA), **f64)
+            self.final_scans = torch.zeros((NA, self.num_beams), dtype=torch.float32, device=dev)
+            self.final_collisions = torch.zeros((NA,), **f64)
+            self.final_collision_idx = torch.full((NA,), -1, dtype=torch.int32, device=dev)
+            self.final_lap_times = torch.zeros((NA,), **f64)
+            self.final_lap_counts = torch.zeros((NA,), **f64)
+            self.ep_list = torch.zeros((N,), dtype=torch.int32, device=dev)
+            self.ep_list_count = torch.zeros((1,), dtype=torch.int32, device=dev)
+        self._episodes = nat.F110Episodes(int(T), nat.ptr(self.ep_ticks), nat.ptr(self.ep_terminated), nat.ptr(self.ep_truncated),
+                                          nat.ptr(self.ep_length), nat.ptr(self.final_state), nat.ptr(self.final_scans),
+                                          nat.ptr(self.final_collisions), nat.ptr(self.final_collision_idx),
+                                          nat.ptr(self.final_lap_times), nat.ptr(self.final_lap_counts), nat.ptr(self.ep_list),
+                                          nat.ptr(self.ep_list_count), None)
+
+    @property
+    def episode_ticks(self):
+        """(N,) int32: ticks of each env's running episode (the restart's zero-action tick does not count)."""
+        return self.ep_ticks
+
+    @property
+    def terminated(self):
+        """(N,) uint8: the env's episode ended on the last episode tick because it was done."""
+        return self.ep_terminated
+
+    @property
+    def truncated(self):
+        """(N,) uint8: the env's episode ended on the last episode tick at the time limit without being done."""
+        return self.ep_truncated
+
+    @property
+    def episode_length(self):
+        """(N,) int32: ticks of each env's last ended episode."""
+        return self.ep_length
+
+    @property
+    def final_observation(self):
+        """The last ended episode's final observation of each env, shaped like observations(): views of the final_* buffers,
+        bit for bit what the tick that ended it left, rewritten only when the env ends another episode."""
+        if self._episodes is None:
+            return None
+        N, A, B = self.num_envs, self.num_agents, self.num_beams
+        st = self.final_state
+        return {'ego_idx': self.ego_idx, 'scans': self.final_scans.view(N, A, B),
+                'poses_x': st[0].view(N, A), 'poses_y': st[1].view(N, A), 'poses_theta': st[4].view(N, A),
+                'linear_vels_x': st[3].view(N, A), 'linear_vels_y': self._zeros_NA, 'ang_vels_z': st[5].view(N, A),
+                'collisions': self.final_collisions.view(N, A), 'collision_idx': self.final_collision_idx.view(N, A),
+                'lap_times': self.final_lap_times.view(N, A), 'lap_counts': self.final_lap_counts.view(N, A)}
+
+    def _episode_path(self, table, env_level):
+        if self._episodes is None or table is None:
+            return False
+        if not env_level:
+            raise ValueError('episode mode needs env_level=True: the end of an episode is decided by done')
+        return True
+
+    def _no_episodes(self, who):
+        if self._episodes is not None:
+            raise ValueError('%s does not run episode mode; call set_episodes(False) first or use tick / capture_graph' % who)
+
+    def _launch_episodes(self, L, actions, table, num_start, pose_gap, seed):
+        self._episodes.track_seg = nat.ptr(self.track_seg)
+        nat.check(L.f110_tick_episodes(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                       C.byref(self.beams.c), nat.ptr(actions), nat.ptr(table), num_start, pose_gap, int(seed),
+                                       self._obst_ref(), self._lidar_ref(), C.byref(self._episodes), _stream_ptr(self.device)))
 
     # ------------------------------------------------------------------ agents without a lidar
     def set_lidar(self, slots):
@@ -795,6 +902,7 @@ class Simulator(object):
         by the next call; both need env_level).  On the ticks before the last only the agents a wall could stop are marched.
         progress=True (needs set_centerlines): update_progress() after every tick of the call; track_delta_sum (N*A,) then
         holds each agent's progress over the whole call."""
+        self._no_episodes('tick_repeat')
         K = self._check_repeat(repeat)
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
@@ -984,12 +1092,15 @@ class Simulator(object):
         stream, march queue history, progress tracker) is restored afterwards, so capturing has no side effect on the
         simulation.  progress=True appends update_progress() to the captured tick (needs set_centerlines).
         repeat > 1 captures tick_repeat(actions, repeat) instead (done_any / done_tick with env_level); with progress=True the
-        tracker is updated after every tick of the call and track_delta_sum (N*A,) holds the sum of the call's deltas."""
+        tracker is updated after every tick of the call and track_delta_sum (N*A,) holds the sum of the call's deltas.
+        With episode mode set (set_episodes), autoreset_poses and env_level=True capture the episode tick instead."""
         assert actions.is_cuda and actions.dtype == torch.float64 and actions.is_contiguous()
         if progress and self.centerlines is None:
             raise ValueError('capture_graph(progress=True) needs set_centerlines first')
         L = nat.lib()
         K = self._check_repeat(repeat)
+        if K > 1:
+            self._no_episodes('capture_graph(repeat > 1)')
         call = self._repeat_call(env_level, progress) if K > 1 else None
         names = ('state', 'steer_buf', 'steer_cnt', 'scan_pose', 'agent_poses', 'scans', 'wall_flag', 'collisions',
                  'collision_idx', 'current_time', 'lap_times', 'lap_counts', 'toggle_list', 'near_starts', 'start_xs',
@@ -997,13 +1108,21 @@ class Simulator(object):
                  'march_order', 'march_count', 'march_rec', 'track_seg', 'track_s', 'track_d', 'track_heading_error',
                  'track_progress', 'track_delta', 'done_any', 'done_tick', 'repeat_list', 'repeat_list_count',
                  'marched_agents', 'track_delta_sum', 'obstacle_boxes', 'obstacle_active', 'obstacle_hit', 'lidar_list',
-                 'lidar_list_count', 'lidar_listed')
+                 'lidar_list_count', 'lidar_listed', 'ep_ticks', 'ep_terminated', 'ep_truncated', 'ep_length', 'final_state',
+                 'final_scans', 'final_collisions', 'final_collision_idx', 'final_lap_times', 'final_lap_counts', 'ep_list',
+                 'ep_list_count')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
+        episodes = self._episode_path(table, env_level)
 
         def tick():
             if K > 1:
                 self._issue_repeat(L, actions, K, call, env_level, table, num_start, pose_gap, autoreset_seed, progress)
+                return
+            if episodes:
+                self._launch_episodes(L, actions, table, num_start, pose_gap, autoreset_seed)
+                if progress:
+                    self._launch_progress(L)
                 return
             nat.check(L.f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
                                         C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
@@ -1027,7 +1146,8 @@ class Simulator(object):
         self._graph_keep = (actions, table) + ((self.centerlines, self._progress_views) if progress else ()) + \
             ((call,) if K > 1 else ()) + ((self._obst, self.obstacle_boxes, self.obstacle_active, self.obstacle_hit) +
                                           self._obst_keep if self._obst is not None else ()) + \
-            ((self._lidar, self.lidar_list, self.lidar_list_count, self.lidar_listed) if self._lidar is not None else ())
+            ((self._lidar, self.lidar_list, self.lidar_list_count, self.lidar_listed) if self._lidar is not None else ()) + \
+            ((self._episodes,) if episodes else ())
         return g
 
     def replay(self):
@@ -1037,6 +1157,7 @@ class Simulator(object):
         """Pinned host buffers for step_host() / step_host_async().  packed_scans=True (async path only): the scan block
         crosses PCIe as 24-bit fixed point (io['scans_u24'] uint8 [NA, B, 3]; decode with unpack_scans_u24) instead of fp32."""
         self._no_lidar_mask('make_host_io')
+        self._no_episodes('make_host_io')
         N, A, B = self.num_envs, self.num_agents, self.num_beams
         NA = N * A
         if packed_scans:
@@ -1065,6 +1186,7 @@ class Simulator(object):
         D2H observation, stream sync.  io from make_host_io(); fill io['actions'] first.  ValueError with obstacles set."""
         self._no_obstacles('step_host')
         self._no_lidar_mask('step_host')
+        self._no_episodes('step_host')
         nat.check(nat.lib().f110_step_host(C.byref(self.c), C.byref(self._map_struct), C.byref(self.beams.c),
                                            nat.ptr(io['actions']), nat.ptr(self._actions_dev),
                                            C.byref(io['_struct']), _stream_ptr(self.device)))
@@ -1076,6 +1198,7 @@ class Simulator(object):
         the scan noise reaches 32 m, where the 24-bit block clamps (step_host_async checks again once the map or the noise
         changed)."""
         self._no_lidar_mask('make_host_pipeline')
+        self._no_episodes('make_host_pipeline')
         N, A, B = self.num_envs, self.num_agents, self.num_beams
         NA = N * A
         dev = self.device
@@ -1125,6 +1248,7 @@ class Simulator(object):
         with obstacles set."""
         self._no_obstacles('step_host_async')
         self._no_lidar_mask('step_host_async')
+        self._no_episodes('step_host_async')
         if io['scans_u24'] is not None:
             checked = io.get('_packed_checked')
             if checked is None or checked[0] is not self._map_struct or checked[1] != self.c.noise_std:
@@ -1146,6 +1270,7 @@ class Simulator(object):
         set."""
         self._no_obstacles('step_profile')
         self._no_lidar_mask('step_profile')
+        self._no_episodes('step_profile')
         a = self._actions_tensor(control_inputs)
         ms = (C.c_float * 3)()
         nat.check(nat.lib().f110_step_profile_ex(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
