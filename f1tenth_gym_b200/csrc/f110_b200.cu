@@ -2870,8 +2870,8 @@ int f110_tick_episodes(const f110_sim *sim, const f110_map *map, const f110_marc
                                                                                           ep->list_count);
         LAUNCH_CHECK("k_episode_obstacles");
     }
-    append_launch_record(" episodes restart=k_episode_end+k_episode_dyn+k_restart_march%s+k_episode_tail%s",
-                         (A > 1 && slots) ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "");
+    append_launch_record(" episodes restart=k_episode_end+k_episode_dyn+k_restart_march%s+k_episode_tail%s restart_grid=%u",
+                         (A > 1 && slots) ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "", grid);
     return F110_OK;
 }
 

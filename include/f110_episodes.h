@@ -56,7 +56,7 @@ typedef struct {
 /* One episode tick.  F110_ERR_INVALID before anything is enqueued for: ep or any of its buffers NULL (track_seg may be),
  * max_ticks < 0, more than 32 agents per env, start_poses NULL, a tick whose ray march is not one of the lean kernels (the
  * restart march shares their arithmetic), and what f110_tick_lidar rejects.  The launch record (f110_debug_last_launch) gains
- * " episodes restart=<kernels>". */
+ * " episodes restart=<kernels> restart_grid=<blocks of k_restart_march>". */
 int f110_tick_episodes(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
                        const double *actions, const double *start_poses, int32_t num_start, int32_t pose_gap, uint64_t seed,
                        const f110_obstacles *obst, const f110_lidar *lidar, const f110_episodes *ep, void *stream);
