@@ -105,6 +105,12 @@ class F110Episodes(C.Structure):
                 ('final_state', _dp), ('final_scans', _dp), ('final_collisions', _dp), ('final_collision_idx', _dp),
                 ('final_lap_times', _dp), ('final_lap_counts', _dp), ('list', _dp), ('list_count', _dp), ('track_seg', _dp)]
 
+
+class F110EpisodeRepeat(C.Structure):
+    """include/f110_episode_repeat.h f110_episode_repeat."""
+    _fields_ = [('end_tick', _dp), ('snap_rec', _dp), ('snap_poses', _dp), ('snap_wall_flag', _dp), ('scan_list', _dp),
+                ('scan_count', _dp), ('track_delta_sum', _dp)]
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol declared
 # in include/f110_b200.h is exported.
 _P = C.POINTER
@@ -185,6 +191,16 @@ EPISODE_SIGNATURES = {
                                      C.c_uint64, _P(F110Obstacles), _P(F110Lidar), _P(F110Episodes), _dp]),
 }
 
+# the entry points of include/f110_episode_repeat.h (episodes under a held action), bound like SIGNATURES
+EPISODE_REPEAT_SIGNATURES = {
+    'f110_tick_repeat_episodes': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32,
+                                            _P(F110Repeat), _dp, C.c_int32, C.c_int32, C.c_uint64, _P(F110Obstacles), _P(F110Lidar),
+                                            _P(F110Episodes), _P(F110EpisodeRepeat), _dp]),
+    'f110_tick_repeat_episodes_ticks': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _dp, C.c_int32,
+                                                  C.c_int32, C.c_int32, _P(F110Repeat), _dp, C.c_int32, C.c_int32, C.c_uint64,
+                                                  _P(F110Obstacles), _P(F110Lidar), _P(F110Episodes), _P(F110EpisodeRepeat), _dp]),
+}
+
 DEBUG_SIGNATURES = {
     'f110_debug_set_variant': (None, [C.c_int]),
     'f110_debug_set_chunk': (None, [C.c_int]),
@@ -224,7 +240,7 @@ def lib():
         L = C.CDLL(LIB_PATH)
     except OSError as e:
         raise NativeLibraryError('f1tenth_gym_b200: cannot load %s: %s' % (LIB_PATH, e))
-    for name, (res, args) in list(SIGNATURES.items()) + list(EPISODE_SIGNATURES.items()):
+    for name, (res, args) in list(SIGNATURES.items()) + list(EPISODE_SIGNATURES.items()) + list(EPISODE_REPEAT_SIGNATURES.items()):
         try:
             f = getattr(L, name)
         except AttributeError:

@@ -29,6 +29,7 @@
 
 #include "../../include/f110_b200.h"
 #include "../../include/f110_episodes.h"
+#include "../../include/f110_episode_repeat.h"
 #include "collision.cuh"
 #include "dynamics.cuh"
 #include "lidar.cuh"
@@ -1148,6 +1149,7 @@ __global__ void __launch_bounds__(32 * F110_LIDAR_CAST_WARPS) k_lidar_cast(f110_
 }  // namespace f110
 #include "obstacles.cuh"     // k_obstacles, k_env_tail_obst: built on the tail's device functions above
 #include "episodes.cuh"      // the restart of ended episodes: built on the same functions and on obstacles.cuh's
+#include "episode_repeat.cuh"   // episodes under a held action: the end latch, reusing the restart kernels above
 namespace f110 {
 
 // f110_track_progress_sum: the deltas of the ticks of one policy step, summed in tick order
@@ -1314,7 +1316,7 @@ static int check_beams(const f110_beams *b) {
 static unsigned long long *g_trace = nullptr;          // debug only: per-block timeline buffer (f110_debug_set_trace)
 static unsigned long long *g_tile_counter = nullptr;   // debug only: lookups served from the shared-memory tile
 // debug record of the kernels the last tick / f110_scan_layers of this thread launched (f110_debug_last_launch): host-side text only
-static thread_local char g_launch_rec[448] = "";
+static thread_local char g_launch_rec[768] = "";
 
 static int num_sms() {
     static int n = 0;
@@ -2944,6 +2946,179 @@ int f110_tick_repeat(const f110_sim *sim, const f110_map *map, const f110_march_
                      int32_t num_start, int32_t pose_gap, uint64_t seed, void *stream) {
     return f110_tick_repeat_ticks(sim, map, tables, beams, actions, repeat, 0, repeat, rep, env_level, start_poses, num_start,
                                   pose_gap, seed, stream);
+}
+
+// ---- episodes under a held action (csrc/episode_repeat.cuh): the ticks of f110_tick_repeat, k_episode_latch after each, then
+// the final scans of the envs that ended on a short-path tick and the restart of every env that ended in the call
+int f110_tick_repeat_episodes_ticks(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables,
+                                    const f110_beams *beams, const double *actions, int32_t repeat, int32_t first_tick,
+                                    int32_t num_ticks, const f110_repeat *rep, const double *start_poses, int32_t num_start,
+                                    int32_t pose_gap, uint64_t seed, const f110_obstacles *obst, const f110_lidar *lidar,
+                                    const f110_episodes *ep, const f110_episode_repeat *er, void *stream) {
+    int rc;
+    TailOpts t;
+    RepeatPlan rp;
+    TickPlan last;           // the last tick of the call: the plain tick's plan, with the lidar mask
+    ObstPlan ob;
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((rc = tick_tail_opts(sim, map, 1, start_poses, num_start, pose_gap, seed, &t))) return rc;
+    if ((rc = check_lidar(sim, lidar))) return rc;
+    if (repeat < 1 || repeat > F110_MAX_REPEAT || first_tick < 0 || num_ticks < 1 || first_tick > repeat - num_ticks) return F110_ERR_INVALID;
+    if (!rep || !rep->list || !rep->list_count) return F110_ERR_INVALID;
+    if ((rc = check_episodes(sim, ep, start_poses))) return rc;
+    if (!er || !er->end_tick || !er->snap_rec || !er->snap_poses || !er->snap_wall_flag || !er->scan_list || !er->scan_count)
+        return F110_ERR_INVALID;
+    const AutoResetArgs ar = t.ar;
+    t.ar.start_poses = nullptr;          // the ticks run without the auto-reset; k_episode_restart restarts the ended envs
+    g_launch_rec[0] = '\0';
+    if ((rc = plan_repeat(sim, map, tables, beams, actions, repeat, &rp))) return rc;
+    if (!episode_march_ok(rp.tick.march)) return F110_ERR_INVALID;
+    const bool masked = lidar && lidar->mask != F110_LIDAR_ALL;
+    if (masked && (rc = plan_tick(sim, map, tables, beams, actions, &last, lidar))) return rc;
+    if (obst) {
+        if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
+        rp.tick.obst = &ob;
+        last.obst = &ob;
+    }
+    TickPlan &lp = masked ? last : rp.tick;
+    if (!episode_march_ok(lp.march)) return F110_ERR_INVALID;      // the plan the last tick and the restart march run with
+    const int units = lp.march.rot ? F110_SCAN_UNITS_ROT : lp.march.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+    unsigned grid = 0u, fs_grid = 0u;
+    if ((rc = units == F110_SCAN_UNITS_ROT ? restart_grid<F110_SCAN_UNITS_ROT>(lp.march.count, &grid)
+            : units == F110_SCAN_UNITS_CELLS ? restart_grid<F110_SCAN_UNITS_CELLS>(lp.march.count, &grid)
+                                             : restart_grid<F110_SCAN_UNITS_METRES>(lp.march.count, &grid)))
+        return rc;
+    if (rp.ttc && (rc = units == F110_SCAN_UNITS_ROT ? restart_grid<F110_SCAN_UNITS_ROT>(false, &fs_grid)
+                       : units == F110_SCAN_UNITS_CELLS ? restart_grid<F110_SCAN_UNITS_CELLS>(false, &fs_grid)
+                                                        : restart_grid<F110_SCAN_UNITS_METRES>(false, &fs_grid)))
+        return rc;
+
+    const int N = sim->num_envs, A = sim->num_agents, NA = N * A;
+    const uint32_t all = A == 32 ? 0xFFFFFFFFu : (1u << A) - 1u;
+    // the slots whose scans the last tick computes, and the slots that have a lidar (their scans go to final_scans)
+    const uint32_t scan_slots = lp.lidar ? lp.lidar->mask : all;
+    const uint32_t final_slots = masked ? (lidar->mask & all) : all;
+    f110_repeat rn = *rep;               // the ticks' own done bookkeeping is off: k_episode_latch keeps it to the running episode
+    rn.done_any = nullptr; rn.done_tick = nullptr;
+    LatchK k;
+    k.ep.ticks = ep->ticks; k.ep.length = ep->length; k.ep.terminated = ep->terminated; k.ep.truncated = ep->truncated;
+    k.ep.final_state = ep->final_state; k.ep.final_collisions = ep->final_collisions; k.ep.final_lap_times = ep->final_lap_times;
+    k.ep.final_lap_counts = ep->final_lap_counts; k.ep.final_collision_idx = ep->final_collision_idx;
+    k.ep.list = ep->list; k.ep.count = ep->list_count; k.ep.track_seg = ep->track_seg; k.ep.max_ticks = ep->max_ticks;
+    k.end_tick = er->end_tick; k.done_any = rep->done_any; k.done_tick = rep->done_tick;
+    k.scans = sim->scans; k.final_scans = ep->final_scans;
+    k.snap_rec = reinterpret_cast<double2 *>(er->snap_rec); k.snap_poses = er->snap_poses; k.snap_flag = er->snap_wall_flag;
+    k.scan_list = er->scan_list; k.scan_count = er->scan_count;
+    k.num_beams = beams->num_beams; k.final_slots = final_slots;
+
+    if (first_tick == 0) {
+        CUDA_TRY(cudaMemsetAsync(rep->list_count, 0, sizeof(uint32_t) * (size_t)repeat, st));
+        CUDA_TRY(cudaMemsetAsync(er->scan_count, 0, sizeof(uint32_t), st));
+    }
+    for (int tick = first_tick; tick < first_tick + num_ticks; tick++) {
+        const bool short_tick = rp.ttc && tick < repeat - 1;
+        if (short_tick) {
+            if ((rc = launch_ttc_tick(sim, map, beams, actions, rp, &rn, tick, t, st))) return rc;
+        } else if ((rc = launch_tick(sim, map, tables, beams, actions, tick == repeat - 1 ? lp : rp.tick, st,
+                                     nullptr, &t))) {
+            return rc;
+        }
+        k.tick = tick;
+        k.scans_exist = short_tick ? 0 : 1;
+        k_episode_latch<<<(unsigned)(((long long)N * 32 + 127) / 128), 128, 0, st>>>(*sim, k);
+        LAUNCH_CHECK("k_episode_latch");
+    }
+    const size_t n = strlen(g_launch_rec);
+    static const char *unit_names[3] = {"cells", "metres", "rot"};
+    snprintf(g_launch_rec + n, sizeof(g_launch_rec) - n, "%srepeat=%d sub=%s UNITS=%s grid=%u", n ? " " : "", (int)repeat,
+             rp.ttc ? "ttc" : "full", unit_names[rp.units], rp.grid);
+    if (first_tick + num_ticks < repeat) return F110_OK;
+
+    const BeamView bv = make_view(beams);
+    const double max_scan = max_scan_range(sim, map);
+    const unsigned fslots = (unsigned)__builtin_popcount(final_slots);
+    // the final scans of the envs that ended on a short-path tick, from the snapshot of their end tick
+    const bool final_pass = rp.ttc && repeat > 1 && fslots;
+    if (final_pass) {
+        f110_sim fs = *sim;
+        fs.agent_poses = er->snap_poses; fs.wall_flag = er->snap_wall_flag; fs.scans = ep->final_scans;
+        fs.collisions = ep->final_collisions; fs.collision_idx = ep->final_collision_idx;
+        TtcK q = fill_ttc_k(sim, map, beams, rp.tick, er->scan_list, er->scan_count);
+        q.rec = reinterpret_cast<const double2 *>(er->snap_rec);
+        q.wall_flag = er->snap_wall_flag;           // never written: the snapshot's iTTC threshold is -inf
+        RestartK r;
+        r.list = er->scan_list; r.count = er->scan_count; r.scans = ep->final_scans; r.final_scans = ep->final_scans;
+        r.tick_counter = sim->tick_counter; r.noise_std = 0.0; r.noise_seed = 0ull;
+        r.lidar = final_slots; r.final_slots = 0u;
+        if (units == F110_SCAN_UNITS_ROT) launch_restart_march_t<F110_SCAN_UNITS_ROT>(q, r, false, fs_grid, st);
+        else if (units == F110_SCAN_UNITS_CELLS) launch_restart_march_t<F110_SCAN_UNITS_CELLS>(q, r, false, fs_grid, st);
+        else launch_restart_march_t<F110_SCAN_UNITS_METRES>(q, r, false, fs_grid, st);
+        LAUNCH_CHECK("k_restart_march");
+        if (A > 1) {
+            const LidarOrder lo = {final_slots, fslots};
+            k_episode_cast<<<(unsigned)(((unsigned long long)N * fslots + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS),
+                             32 * F110_LIDAR_CAST_WARPS, 0, st>>>(fs, bv, lo, er->scan_list, er->scan_count, max_scan);
+            LAUNCH_CHECK("k_episode_cast");
+        }
+        if (obst) {
+            ObstK o = ob.k;
+            o.lidar = final_slots;
+            o.hit = nullptr;
+            k_episode_obstacles<<<(unsigned)(((long long)NA * 32 + 127) / 128), 128, 0, st>>>(fs, bv, o, max_scan, er->scan_list,
+                                                                                              er->scan_count);
+            LAUNCH_CHECK("k_episode_obstacles");
+        }
+    }
+
+    // the restart of every env that ended in the call, at the counter of its last tick
+    ObstDraw no_draw;
+    memset(&no_draw, 0, sizeof(no_draw));
+    CUDA_TRY(cudaMemsetAsync(ep->list_count, 0, sizeof(uint32_t), st));
+    k_episode_restart<<<(N + 127) / 128, 128, 0, st>>>(*sim, ar, k, obst ? ob.d : no_draw, ep->track_seg, er->track_delta_sum,
+                                                      ep->list, ep->list_count);
+    LAUNCH_CHECK("k_episode_restart");
+    k_episode_dyn<<<(NA + 127) / 128, 128, 0, st>>>(*sim, beams->fov, (double)map->theta_dis,
+                                                    fill_first_lookup(sim, map, beams, lp.geom, lp.march), ep->list, ep->list_count);
+    LAUNCH_CHECK("k_episode_dyn");
+    RestartK r;
+    r.list = ep->list; r.count = ep->list_count; r.scans = sim->scans; r.final_scans = ep->final_scans;
+    r.tick_counter = sim->tick_counter; r.noise_std = sim->noise_std; r.noise_seed = sim->noise_seed;
+    r.lidar = scan_slots; r.final_slots = 0u;    // the crash scans are in final_scans already (k_episode_latch)
+    const TtcK q = fill_ttc_k(sim, map, beams, lp, ep->list, ep->list_count);
+    if (units == F110_SCAN_UNITS_ROT) launch_restart_march_t<F110_SCAN_UNITS_ROT>(q, r, lp.march.count, grid, st);
+    else if (units == F110_SCAN_UNITS_CELLS) launch_restart_march_t<F110_SCAN_UNITS_CELLS>(q, r, lp.march.count, grid, st);
+    else launch_restart_march_t<F110_SCAN_UNITS_METRES>(q, r, lp.march.count, grid, st);
+    LAUNCH_CHECK("k_restart_march");
+    const unsigned slots = (unsigned)__builtin_popcount(scan_slots);
+    if (A > 1 && slots) {
+        const LidarOrder lo = {scan_slots, slots};
+        k_episode_cast<<<(unsigned)(((unsigned long long)N * slots + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS),
+                         32 * F110_LIDAR_CAST_WARPS, 0, st>>>(*sim, bv, lo, ep->list, ep->list_count, max_scan);
+        LAUNCH_CHECK("k_episode_cast");
+    }
+    k_episode_tail<<<(N + 127) / 128, 128, 0, st>>>(*sim, ep->list, ep->list_count);
+    LAUNCH_CHECK("k_episode_tail");
+    if (obst) {
+        ObstK o = ob.k;
+        o.lidar = scan_slots;
+        k_episode_obstacles<<<(unsigned)(((long long)NA * 32 + 127) / 128), 128, 0, st>>>(*sim, bv, o, max_scan, ep->list,
+                                                                                          ep->list_count);
+        LAUNCH_CHECK("k_episode_obstacles");
+    }
+    append_launch_record(" episodes restart=k_episode_restart+k_episode_dyn+k_restart_march%s+k_episode_tail%s restart_grid=%u",
+                         (A > 1 && slots) ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "", grid);
+    if (final_pass)
+        append_launch_record(" final_scan=k_restart_march%s%s", A > 1 ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "");
+    else
+        append_launch_record(" final_scan=none");
+    return F110_OK;
+}
+int f110_tick_repeat_episodes(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                              const double *actions, int32_t repeat, const f110_repeat *rep, const double *start_poses,
+                              int32_t num_start, int32_t pose_gap, uint64_t seed, const f110_obstacles *obst,
+                              const f110_lidar *lidar, const f110_episodes *ep, const f110_episode_repeat *er, void *stream) {
+    return f110_tick_repeat_episodes_ticks(sim, map, tables, beams, actions, repeat, 0, repeat, rep, start_poses, num_start,
+                                           pose_gap, seed, obst, lidar, ep, er, stream);
 }
 
 int f110_step_host(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions_host,

@@ -41,6 +41,13 @@ observation obs holds for that env.  done = terminated | truncated; info adds 't
 'final_observation' (the ended episode's last observation: state keys, scans, collisions, lap_times, lap_counts).  All are
 views of device buffers, overwritten by the next step.  local_map and the progress keys are those after the restart; with
 reward='progress' a restarted env earns 0 on that step.  reset() and reset_envs() zero the episode counters.
+autoreset={..., 'action_repeat': K} (Simulator.tick_repeat in episode mode) holds each action for K ticks, and an env's episode
+stops at the first of them that ends it, as a frame-skip wrapper that stops at done would: its final_observation, flags and
+done are that tick's, and it restarts after the call.  T counts step() calls (a time limit of T * K ticks); info also gets
+'end_tick' (the tick 0..K-1 at which the episode ended, -1 = none) and episode_length is in step() calls (ceil(ticks / K)).
+The reward is (end_tick + 1) * timestep for an env that ended and K * timestep otherwise, (N,) on the device; with
+reward='progress' a restarted env earns 0 and the others the sum of the ego's K deltas.  The top-level action_repeat, which
+runs straight through an env's end, cannot be combined with autoreset.
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
@@ -116,7 +123,7 @@ class F110Env(object):
         if lidar is not None:
             self.sim.set_lidar(lidar)
         if self._autoreset is not None:
-            self.sim.set_episodes(self._autoreset['max_episode_steps'])
+            self.sim.set_episodes(self._autoreset['max_episode_steps'] * self._autoreset['action_repeat'])
             p = self._autoreset['poses']
             self._autoreset['poses'] = [t.to(self.sim.device) for t in p] if isinstance(p, list) else p.to(self.sim.device).contiguous()
         if self._obstacles is not None:
@@ -233,6 +240,8 @@ class F110Env(object):
             return self._step_repeat(action)
         if not self.batched:
             return self._step_single(action)
+        if self._autoreset is not None and self._autoreset['action_repeat'] > 1:
+            return self._step_episode_repeat(action)
         if self._autoreset is not None:
             ar = self._autoreset
             obs = self.sim.tick(action, env_level=True, autoreset_poses=ar['poses'], pose_gap=ar['pose_gap'], seed=ar['seed'])
@@ -268,6 +277,33 @@ class F110Env(object):
         return o, reward, bool(done[0].item()), {'checkpoint_done': info['checkpoint_done'][0].cpu().numpy(),
                                                 'done_tick': int(done_tick[0].item())}
 
+    def _step_episode_repeat(self, action):
+        """Batched episode mode with autoreset['action_repeat'] = K: one Simulator.tick_repeat call in episode mode."""
+        sim, ar, N, A = self.sim, self._autoreset, self.num_envs, self.num_agents
+        K = ar['action_repeat']
+        tracked = self.centerline is not None
+        a = action if torch.is_tensor(action) else np.asarray(action, dtype=np.float64).reshape(N, A, 2)
+        obs = sim.tick_repeat(a, K, env_level=True, autoreset_poses=ar['poses'], pose_gap=ar['pose_gap'], seed=ar['seed'],
+                              progress=tracked)
+        obs['lap_times'], obs['lap_counts'] = sim.lap_times.view(N, A), sim.lap_counts.view(N, A)
+        self._obstacle_obs(obs)
+        if self._local_map is not None:
+            obs['local_map'] = self._render_local_map()
+        for k in ('done_any', 'done_tick'):
+            obs.pop(k)
+        term, trunc, end_tick = obs.pop('terminated').bool(), obs.pop('truncated').bool(), obs.pop('end_tick')
+        # the ticks the env spent in its episode during the step
+        reward = torch.where(end_tick >= 0, end_tick + 1, K).to(torch.float64) * self.timestep
+        if tracked:
+            for k, v in PROGRESS_KEYS:
+                obs[k] = sim._progress_views[v]
+            if self.reward_kind == 'progress':
+                reward = sim.track_delta_sum.view(N, A)[:, self.ego_idx].clone()
+        info = {'checkpoint_done': sim.checkpoint_done.view(N, A).bool(), 'terminated': term, 'truncated': trunc,
+                'end_tick': end_tick, 'episode_length': (sim.episode_length + (K - 1)) // K,
+                'final_observation': sim.final_observation}
+        return obs, reward, term | trunc, info
+
     def reset(self, poses):
         """f110_env.py:306-349: zero counters, start frame, Simulator.reset, then ONE zero-action tick
         whose (obs, reward, done, info) is returned."""
@@ -287,21 +323,28 @@ class F110Env(object):
             self.sim.respawn_obstacles(env_mask)
 
     def _autoreset_settings(self, cfg, batched, action_repeat):
-        """autoreset kwarg -> {'poses': device table or list, 'max_episode_steps', 'seed', 'pose_gap'}, or None; ValueError
-        before any device work."""
+        """autoreset kwarg -> {'poses': device table or list, 'max_episode_steps', 'seed', 'pose_gap', 'action_repeat'}, or
+        None; ValueError before any device work."""
         if cfg is None:
             return None
         if not batched:
             raise ValueError('autoreset needs the batched mode (num_envs)')
         if action_repeat != 1:
-            raise ValueError('autoreset runs with action_repeat=1 only')
-        if not isinstance(cfg, dict) or 'poses' not in cfg or set(cfg) - {'poses', 'max_episode_steps', 'seed', 'pose_gap'}:
-            raise ValueError("autoreset must be a dict with 'poses' and optionally 'max_episode_steps', 'seed', 'pose_gap', got %r"
-                             % (cfg,))
+            raise ValueError("autoreset takes the held action as autoreset={..., 'action_repeat': K}, which ends each episode at "
+                             'its own tick; the top-level action_repeat runs through an env\'s end and must stay 1')
+        keys = {'poses', 'max_episode_steps', 'seed', 'pose_gap', 'action_repeat'}
+        if not isinstance(cfg, dict) or 'poses' not in cfg or set(cfg) - keys:
+            raise ValueError("autoreset must be a dict with 'poses' and optionally 'max_episode_steps', 'seed', 'pose_gap', "
+                             "'action_repeat', got %r" % (cfg,))
         T = cfg.get('max_episode_steps', None)
         T = 0 if T is None else T
         if isinstance(T, bool) or int(T) != T or int(T) < 0:
             raise ValueError('autoreset max_episode_steps must be None or an int >= 0, got %r' % (T,))
+        K = cfg.get('action_repeat', 1)
+        if isinstance(K, bool) or not isinstance(K, (int, float, np.integer)) or int(K) != K or not 1 <= int(K) <= 64:
+            raise ValueError('autoreset action_repeat must be an int in [1, 64], got %r' % (K,))
+        if int(T) * int(K) > 0x7FFFFFFF:
+            raise ValueError('autoreset max_episode_steps * action_repeat must fit in int32, got %r * %r' % (T, K))
         poses = cfg['poses']
         tables = poses if isinstance(poses, (list, tuple)) else [poses]
         for t in tables:
@@ -311,7 +354,7 @@ class F110Env(object):
         to_dev = lambda t: torch.as_tensor(np.asarray(t.cpu() if torch.is_tensor(t) else t, dtype=np.float64))
         table = [to_dev(t) for t in poses] if isinstance(poses, (list, tuple)) else to_dev(poses)
         return {'poses': table, 'max_episode_steps': int(T), 'seed': int(cfg.get('seed', 12345)),
-                'pose_gap': int(cfg.get('pose_gap', 23))}
+                'pose_gap': int(cfg.get('pose_gap', 23)), 'action_repeat': int(K)}
 
     def _obstacle_obs(self, obs):
         if self._obstacles is not None:

@@ -423,6 +423,10 @@ class Simulator(object):
         self.ep_ticks = self.ep_terminated = self.ep_truncated = self.ep_length = None
         self.final_state = self.final_scans = self.final_collisions = self.final_collision_idx = None
         self.final_lap_times = self.final_lap_counts = self.ep_list = self.ep_list_count = None
+        # ... and its part under a held action (C ABI f110_episode_repeat)
+        self._episode_repeat = None
+        self.ep_end_tick = self.ep_snap_rec = self.ep_snap_poses = self.ep_snap_wall_flag = None
+        self.ep_scan_list = self.ep_scan_count = None
 
     # ------------------------------------------------------------------ configuration
     def set_map(self, map_path, map_ext, edt='scipy'):
@@ -625,6 +629,9 @@ class Simulator(object):
             self.ep_ticks = self.ep_terminated = self.ep_truncated = self.ep_length = None
             self.final_state = self.final_scans = self.final_collisions = self.final_collision_idx = None
             self.final_lap_times = self.final_lap_counts = self.ep_list = self.ep_list_count = None
+            self.ep_end_tick = self.ep_snap_rec = self.ep_snap_poses = self.ep_snap_wall_flag = None
+            self.ep_scan_list = self.ep_scan_count = None
+            self._episode_repeat = None
             return
         T = 0 if max_ticks is None else max_ticks
         if isinstance(T, bool) or int(T) != T or int(T) < 0 or int(T) > 0x7FFFFFFF:
@@ -646,6 +653,16 @@ class Simulator(object):
             self.final_lap_counts = torch.zeros((NA,), **f64)
             self.ep_list = torch.zeros((N,), dtype=torch.int32, device=dev)
             self.ep_list_count = torch.zeros((1,), dtype=torch.int32, device=dev)
+            # episodes under a held action (tick_repeat / capture_graph with repeat > 1)
+            self.ep_end_tick = torch.full((N,), -1, dtype=torch.int32, device=dev)
+            self.ep_snap_rec = torch.zeros((NA, 8), **f64)
+            self.ep_snap_poses = torch.zeros((NA, 5), **f64)
+            self.ep_snap_wall_flag = torch.zeros((NA,), dtype=torch.int32, device=dev)
+            self.ep_scan_list = torch.zeros((N,), dtype=torch.int32, device=dev)
+            self.ep_scan_count = torch.zeros((1,), dtype=torch.int32, device=dev)
+            self._episode_repeat = nat.F110EpisodeRepeat(nat.ptr(self.ep_end_tick), nat.ptr(self.ep_snap_rec),
+                                                         nat.ptr(self.ep_snap_poses), nat.ptr(self.ep_snap_wall_flag),
+                                                         nat.ptr(self.ep_scan_list), nat.ptr(self.ep_scan_count), None)
         self._episodes = nat.F110Episodes(int(T), nat.ptr(self.ep_ticks), nat.ptr(self.ep_terminated), nat.ptr(self.ep_truncated),
                                           nat.ptr(self.ep_length), nat.ptr(self.final_state), nat.ptr(self.final_scans),
                                           nat.ptr(self.final_collisions), nat.ptr(self.final_collision_idx),
@@ -666,6 +683,11 @@ class Simulator(object):
     def truncated(self):
         """(N,) uint8: the env's episode ended on the last episode tick at the time limit without being done."""
         return self.ep_truncated
+
+    @property
+    def end_tick(self):
+        """(N,) int32: the tick 0..K-1 of the last tick_repeat call in episode mode at which the env's episode ended, -1 = none."""
+        return self.ep_end_tick
 
     @property
     def episode_length(self):
@@ -868,14 +890,24 @@ class Simulator(object):
             raise ValueError('repeat must be an int in [1, %d], got %r' % (nat.MAX_REPEAT, repeat))
         return int(repeat)
 
-    def _issue_repeat(self, L, actions, K, call, env_level, table, num_start, pose_gap, seed, progress):
-        """Enqueue one f110_tick_repeat call; progress: the tracker is updated after every tick of the call (the same ticks,
-        issued one by one) and track_delta_sum gets the sum of the call's deltas."""
+    def _issue_repeat(self, L, actions, K, call, env_level, table, num_start, pose_gap, seed, progress, episodes=False):
+        """Enqueue one f110_tick_repeat call (f110_tick_repeat_episodes with episodes=True); progress: the tracker is updated
+        after every tick of the call (the same ticks, issued one by one) and track_delta_sum gets the sum of the call's deltas."""
         def ticks(first, count):
+            if episodes:
+                nat.check(L.f110_tick_repeat_episodes_ticks(
+                    C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables), C.byref(self.beams.c),
+                    nat.ptr(actions), K, first, count, C.byref(call), nat.ptr(table), num_start, pose_gap, int(seed),
+                    self._obst_ref(), self._lidar_ref(), C.byref(self._episodes), C.byref(self._episode_repeat),
+                    _stream_ptr(self.device)))
+                return
             nat.check(L.f110_tick_repeat_ticks_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
                                                      C.byref(self.beams.c), nat.ptr(actions), K, first, count, C.byref(call),
                                                      1 if env_level else 0, nat.ptr(table), num_start, pose_gap, int(seed),
                                                      self._obst_ref(), self._lidar_ref(), _stream_ptr(self.device)))
+        if episodes:
+            self._episodes.track_seg = nat.ptr(self.track_seg)
+            self._episode_repeat.track_delta_sum = nat.ptr(self.track_delta_sum) if progress else None
         if not progress:
             ticks(0, K)
             return
@@ -901,18 +933,28 @@ class Simulator(object):
         an env was done on any tick of the call, and 'done_tick' (N,) int32, the first such tick or -1 (device views, overwritten
         by the next call; both need env_level).  On the ticks before the last only the agents a wall could stop are marched.
         progress=True (needs set_centerlines): update_progress() after every tick of the call; track_delta_sum (N*A,) then
-        holds each agent's progress over the whole call."""
-        self._no_episodes('tick_repeat')
+        holds each agent's progress over the whole call.
+        In episode mode (set_episodes) with autoreset_poses and env_level (C ABI f110_tick_repeat_episodes): an env's episode
+        stops at the first tick of the call that ends it; its final_observation, episode_length and flags are that tick's, done
+        is that tick's and done_any / done_tick count the ticks up to it; after the call it is restarted as tick() restarts it.
+        The other envs are what tick_repeat leaves.  Adds 'terminated', 'truncated' and 'end_tick' (the tick 0..K-1 at which
+        the episode ended, -1 = none); with progress=True a restarted env's track_delta_sum is 0.  Episode mode without
+        autoreset_poses raises ValueError."""
         K = self._check_repeat(repeat)
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
+        episodes = self._episode_path(table, env_level)
+        if not episodes:
+            self._no_episodes('tick_repeat without autoreset_poses')
         call = self._repeat_call(env_level, progress)
-        self._issue_repeat(nat.lib(), a, K, call, env_level, table, n, pose_gap, seed, progress)
+        self._issue_repeat(nat.lib(), a, K, call, env_level, table, n, pose_gap, seed, progress, episodes)
         self._repeat_ticks += (K - 1) * self.num_envs * self.num_agents
         self._repeat_plain = b'sub=full' in nat.lib().f110_debug_last_launch()      # the call ran plain ticks throughout
         obs = self.observations()
         if env_level:
             obs['done_any'], obs['done_tick'] = self.done_any, self.done_tick
+        if episodes:
+            obs['terminated'], obs['truncated'], obs['end_tick'] = self.ep_terminated, self.ep_truncated, self.ep_end_tick
         return obs
 
     def marched_fraction(self):
@@ -1093,14 +1135,15 @@ class Simulator(object):
         simulation.  progress=True appends update_progress() to the captured tick (needs set_centerlines).
         repeat > 1 captures tick_repeat(actions, repeat) instead (done_any / done_tick with env_level); with progress=True the
         tracker is updated after every tick of the call and track_delta_sum (N*A,) holds the sum of the call's deltas.
-        With episode mode set (set_episodes), autoreset_poses and env_level=True capture the episode tick instead."""
+        With episode mode set (set_episodes), autoreset_poses and env_level=True capture the episode tick instead, and with
+        repeat > 1 the episode call of tick_repeat."""
         assert actions.is_cuda and actions.dtype == torch.float64 and actions.is_contiguous()
         if progress and self.centerlines is None:
             raise ValueError('capture_graph(progress=True) needs set_centerlines first')
         L = nat.lib()
         K = self._check_repeat(repeat)
-        if K > 1:
-            self._no_episodes('capture_graph(repeat > 1)')
+        if K > 1 and (autoreset_poses is None or not env_level):
+            self._no_episodes('capture_graph(repeat > 1) without autoreset_poses and env_level')
         call = self._repeat_call(env_level, progress) if K > 1 else None
         names = ('state', 'steer_buf', 'steer_cnt', 'scan_pose', 'agent_poses', 'scans', 'wall_flag', 'collisions',
                  'collision_idx', 'current_time', 'lap_times', 'lap_counts', 'toggle_list', 'near_starts', 'start_xs',
@@ -1110,14 +1153,15 @@ class Simulator(object):
                  'marched_agents', 'track_delta_sum', 'obstacle_boxes', 'obstacle_active', 'obstacle_hit', 'lidar_list',
                  'lidar_list_count', 'lidar_listed', 'ep_ticks', 'ep_terminated', 'ep_truncated', 'ep_length', 'final_state',
                  'final_scans', 'final_collisions', 'final_collision_idx', 'final_lap_times', 'final_lap_counts', 'ep_list',
-                 'ep_list_count')
+                 'ep_list_count', 'ep_end_tick', 'ep_snap_rec', 'ep_snap_poses', 'ep_snap_wall_flag', 'ep_scan_list',
+                 'ep_scan_count')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
         episodes = self._episode_path(table, env_level)
 
         def tick():
             if K > 1:
-                self._issue_repeat(L, actions, K, call, env_level, table, num_start, pose_gap, autoreset_seed, progress)
+                self._issue_repeat(L, actions, K, call, env_level, table, num_start, pose_gap, autoreset_seed, progress, episodes)
                 return
             if episodes:
                 self._launch_episodes(L, actions, table, num_start, pose_gap, autoreset_seed)
@@ -1147,7 +1191,7 @@ class Simulator(object):
             ((call,) if K > 1 else ()) + ((self._obst, self.obstacle_boxes, self.obstacle_active, self.obstacle_hit) +
                                           self._obst_keep if self._obst is not None else ()) + \
             ((self._lidar, self.lidar_list, self.lidar_list_count, self.lidar_listed) if self._lidar is not None else ()) + \
-            ((self._episodes,) if episodes else ())
+            ((self._episodes,) if episodes else ()) + ((self._episode_repeat,) if episodes and K > 1 else ())
         return g
 
     def replay(self):
