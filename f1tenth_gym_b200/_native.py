@@ -111,6 +111,16 @@ class F110EpisodeRepeat(C.Structure):
     _fields_ = [('end_tick', _dp), ('snap_rec', _dp), ('snap_poses', _dp), ('snap_wall_flag', _dp), ('scan_list', _dp),
                 ('scan_count', _dp), ('track_delta_sum', _dp)]
 
+
+class F110ParamDraw(C.Structure):
+    """include/f110_param_draw.h f110_param_draw."""
+    _fields_ = [('lo', _dp), ('hi', _dp), ('keys', C.c_uint32 * 32), ('group', C.c_int32 * F110_NPARAM), ('per_env', C.c_int32),
+                ('seed', C.c_uint64), ('final_params', _dp)]
+
+
+PARAM_DRAW_KEYS = 16     # keys 0..15 are drawable; width and length are not
+PARAM_DRAW_C = (0xC2B2AE3D27D4EB4F, 0x165667B19E3779F9, 0x27D4EB2F165667C5, 0x85EBCA77C2B2AE63)   # C1..C4 (tick, env, slot, group)
+
 # name -> (restype, argtypes); this table is also what tests use to check that every symbol declared
 # in include/f110_b200.h is exported.
 _P = C.POINTER
@@ -201,6 +211,13 @@ EPISODE_REPEAT_SIGNATURES = {
                                                   _P(F110Obstacles), _P(F110Lidar), _P(F110Episodes), _P(F110EpisodeRepeat), _dp]),
 }
 
+# the entry points of include/f110_param_draw.h (per-episode parameter draws), bound like SIGNATURES
+PARAM_DRAW_SIGNATURES = {
+    'f110_params_draw': (C.c_int, [_P(F110Sim), _P(F110ParamDraw), _dp, _dp]),
+    'f110_params_draw_autoreset': (C.c_int, [_P(F110Sim), _P(F110ParamDraw), _dp]),
+    'f110_params_draw_episodes': (C.c_int, [_P(F110Sim), _P(F110ParamDraw), _P(F110Episodes), _dp]),
+}
+
 DEBUG_SIGNATURES = {
     'f110_debug_set_variant': (None, [C.c_int]),
     'f110_debug_set_chunk': (None, [C.c_int]),
@@ -240,7 +257,8 @@ def lib():
         L = C.CDLL(LIB_PATH)
     except OSError as e:
         raise NativeLibraryError('f1tenth_gym_b200: cannot load %s: %s' % (LIB_PATH, e))
-    for name, (res, args) in list(SIGNATURES.items()) + list(EPISODE_SIGNATURES.items()) + list(EPISODE_REPEAT_SIGNATURES.items()):
+    for name, (res, args) in list(SIGNATURES.items()) + list(EPISODE_SIGNATURES.items()) + list(EPISODE_REPEAT_SIGNATURES.items()) + \
+            list(PARAM_DRAW_SIGNATURES.items()):
         try:
             f = getattr(L, name)
         except AttributeError:

@@ -30,6 +30,7 @@
 #include "../../include/f110_b200.h"
 #include "../../include/f110_episodes.h"
 #include "../../include/f110_episode_repeat.h"
+#include "../../include/f110_param_draw.h"
 #include "collision.cuh"
 #include "dynamics.cuh"
 #include "lidar.cuh"
@@ -1150,6 +1151,7 @@ __global__ void __launch_bounds__(32 * F110_LIDAR_CAST_WARPS) k_lidar_cast(f110_
 #include "obstacles.cuh"     // k_obstacles, k_env_tail_obst: built on the tail's device functions above
 #include "episodes.cuh"      // the restart of ended episodes: built on the same functions and on obstacles.cuh's
 #include "episode_repeat.cuh"   // episodes under a held action: the end latch, reusing the restart kernels above
+#include "param_draw.cuh"       // per-episode parameter draws, launched after the call that restarted the envs
 namespace f110 {
 
 // f110_track_progress_sum: the deltas of the ticks of one policy step, summed in tick order
@@ -3119,6 +3121,47 @@ int f110_tick_repeat_episodes(const f110_sim *sim, const f110_map *map, const f1
                               const f110_lidar *lidar, const f110_episodes *ep, const f110_episode_repeat *er, void *stream) {
     return f110_tick_repeat_episodes_ticks(sim, map, tables, beams, actions, repeat, 0, repeat, rep, start_poses, num_start,
                                            pose_gap, seed, obst, lidar, ep, er, stream);
+}
+
+// ---- per-episode parameter draws (csrc/param_draw.cuh): one k_param_draw launch, after the call that restarted the envs
+static int param_draw_launch(const f110_sim *sim, const f110_param_draw *draw, int rule, const uint8_t *mask,
+                             const f110_episodes *ep, void *stream) {
+    if (!sim || !draw || !draw->lo || !draw->hi) return F110_ERR_INVALID;
+    if (sim->num_envs <= 0 || sim->num_agents <= 0 || sim->num_agents > 32 || !sim->params || !sim->params_per_env ||
+        !sim->tick_counter)
+        return F110_ERR_INVALID;
+    if (rule == PARAM_DRAW_AUTORESET && (!sim->collisions || sim->ego_idx < 0 || sim->ego_idx >= sim->num_agents))
+        return F110_ERR_INVALID;
+    if (rule == PARAM_DRAW_EPISODES && (!ep || !ep->terminated || !ep->truncated)) return F110_ERR_INVALID;
+    const int A = sim->num_agents;
+    for (int i = 0; i < A; i++)
+        if (draw->keys[i] >> F110_PARAM_DRAW_KEYS) return F110_ERR_INVALID;
+    for (int q = 0; q < F110_NPARAM; q++)
+        if (draw->group[q] < 0 || draw->group[q] >= F110_NPARAM) return F110_ERR_INVALID;
+    ParamDrawK k;
+    k.lo = draw->lo; k.hi = draw->hi;
+    k.params = const_cast<double *>(sim->params);
+    k.final_params = rule == PARAM_DRAW_EPISODES ? draw->final_params : nullptr;
+    k.tick_counter = sim->tick_counter;
+    k.mask = mask; k.collisions = sim->collisions;
+    k.terminated = ep ? ep->terminated : nullptr; k.truncated = ep ? ep->truncated : nullptr;
+    k.seed = draw->seed;
+    k.num_envs = sim->num_envs; k.num_agents = A; k.ego = sim->ego_idx; k.rule = rule; k.per_env = draw->per_env ? 1 : 0;
+    memcpy(k.keys, draw->keys, sizeof(k.keys));
+    memcpy(k.group, draw->group, sizeof(k.group));
+    const long long NA = (long long)sim->num_envs * A;
+    k_param_draw<<<(unsigned)((NA + 127) / 128), 128, 0, (cudaStream_t)stream>>>(k);
+    LAUNCH_CHECK("k_param_draw");
+    return F110_OK;
+}
+int f110_params_draw(const f110_sim *sim, const f110_param_draw *draw, const uint8_t *env_mask, void *stream) {
+    return param_draw_launch(sim, draw, PARAM_DRAW_MASK, env_mask, nullptr, stream);
+}
+int f110_params_draw_autoreset(const f110_sim *sim, const f110_param_draw *draw, void *stream) {
+    return param_draw_launch(sim, draw, PARAM_DRAW_AUTORESET, nullptr, nullptr, stream);
+}
+int f110_params_draw_episodes(const f110_sim *sim, const f110_param_draw *draw, const f110_episodes *ep, void *stream) {
+    return param_draw_launch(sim, draw, PARAM_DRAW_EPISODES, nullptr, ep, stream);
 }
 
 int f110_step_host(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions_host,

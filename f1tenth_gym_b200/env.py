@@ -48,12 +48,17 @@ done are that tick's, and it restarts after the call.  T counts step() calls (a 
 The reward is (end_tick + 1) * timestep for an env that ended and K * timestep otherwise, (N,) on the device; with
 reward='progress' a restarted env earns 0 and the others the sum of the ego's K deltas.  The top-level action_repeat, which
 runs straight through an env's end, cannot be combined with autoreset.
+param_draw={'ranges': {key: (lo, hi)} or one dict per agent, 'groups': [['m', 'I']], 'per_env': bool, 'seed': s} (batched mode
+only; Simulator.set_param_draw): per-episode dynamics randomisation.  reset() draws every env's car after placing the agents,
+reset_envs() the masked envs', and the autoreset modes draw every env they restart on the device; info['params'] is the (N, A, 18)
+parameter table after the step (maps.PARAM_KEYS order), i.e. a restarted env's new car.
 The gym 0.19 API with the non-standard reset(poses) is kept on purpose (SURVEY.md 8b).
 """
 import numpy as np
 import torch
 
 from . import maps as hostmaps
+from . import param_draw as pdraw
 from .simulator import RENDER_MAX_AGENTS, Integrator, Simulator
 
 # observation key -> Simulator.update_progress view (added with the centerline kwarg)
@@ -100,6 +105,8 @@ class F110Env(object):
                 raise ValueError('lidar needs one bool per agent (%d), got %d' % (self.num_agents, len(lidar)))
         self._autoreset = self._autoreset_settings(kwargs.get('autoreset', None), self.batched,
                                                    kwargs.get('action_repeat', 1))
+        self._param_draw = self._param_draw_settings(kwargs.get('param_draw', None), self.batched, self.params,
+                                                     self.num_agents)
         self.start_thresh = 0.5
         self.sim = Simulator(self.params, self.num_agents, self.seed, time_step=self.timestep,
                              ego_idx=self.ego_idx, integrator=self.integrator, lidar_dist=self.lidar_dist,
@@ -126,6 +133,9 @@ class F110Env(object):
             self.sim.set_episodes(self._autoreset['max_episode_steps'] * self._autoreset['action_repeat'])
             p = self._autoreset['poses']
             self._autoreset['poses'] = [t.to(self.sim.device) for t in p] if isinstance(p, list) else p.to(self.sim.device).contiguous()
+        if self._param_draw is not None:
+            cfg = self._param_draw
+            self.sim.set_param_draw(cfg['ranges'], cfg.get('groups'), cfg.get('per_env', False), cfg.get('seed', 0))
         if self._obstacles is not None:
             cand, count, clearance, seed = self._obstacles
             self.sim.set_obstacles(np.zeros((count[1], 5)), np.zeros(count[1], bool))
@@ -188,6 +198,7 @@ class F110Env(object):
                 done = term | trunc
                 info.update(terminated=term, truncated=trunc, episode_length=sim.episode_length,
                             final_observation=sim.final_observation)
+            self._param_info(info)
             return obs, reward, done, info
         # single-env, reference-shaped (base_classes.py:594-612): lists of per-agent values
         o = {'ego_idx': obs['ego_idx'],
@@ -267,6 +278,7 @@ class F110Env(object):
         done, done_tick = obs.pop('done_any').bool(), obs.pop('done_tick')
         info = {'checkpoint_done': sim.checkpoint_done.view(N, A).bool(), 'done_tick': done_tick}
         if self.batched:
+            self._param_info(info)
             return obs, reward, done, info
         # single env, reference-shaped: lists of per-agent values
         o = {k: (v if k == 'ego_idx' else v[0].cpu().numpy()) for k, v in obs.items()}
@@ -302,6 +314,7 @@ class F110Env(object):
         info = {'checkpoint_done': sim.checkpoint_done.view(N, A).bool(), 'terminated': term, 'truncated': trunc,
                 'end_tick': end_tick, 'episode_length': (sim.episode_length + (K - 1)) // K,
                 'final_observation': sim.final_observation}
+        self._param_info(info)
         return obs, reward, term | trunc, info
 
     def reset(self, poses):
@@ -310,17 +323,45 @@ class F110Env(object):
         self.sim.env_reset(poses)
         if self._obstacles is not None:
             self.sim.respawn_obstacles()
+        if self._param_draw is not None:
+            self.sim.redraw_params()
         action = torch.zeros((self.num_envs, self.num_agents, 2), dtype=torch.float64, device=self.sim.device)
         if not self.batched:
             return self._step_single(action)
         return self._finish(self.sim.step(action))
 
     def reset_envs(self, env_mask, poses):
-        """Batch extension: re-initialise only the masked envs (counters + Simulator.reset, then their obstacles are redrawn);
-        no tick is run."""
+        """Batch extension: re-initialise only the masked envs (counters + Simulator.reset, then their obstacles and, with
+        param_draw, their cars are redrawn); no tick is run."""
         self.sim.env_reset(poses, env_mask)
         if self._obstacles is not None:
             self.sim.respawn_obstacles(env_mask)
+        if self._param_draw is not None:
+            self.sim.redraw_params(env_mask)
+
+    def _param_info(self, info):
+        if self._param_draw is not None:
+            info['params'] = self.sim.param_table
+
+    @staticmethod
+    def _param_draw_settings(cfg, batched, params, num_agents):
+        """param_draw kwarg -> the dict, validated (param_draw.parse, and the sign conditions on the undrawn values of
+        `params`), or None; ValueError before any device work."""
+        if cfg is None:
+            return None
+        if not batched:
+            raise ValueError('param_draw needs the batched mode (num_envs)')
+        if not isinstance(cfg, dict) or 'ranges' not in cfg or set(cfg) - {'ranges', 'groups', 'per_env', 'seed'}:
+            raise ValueError("param_draw must be a dict with 'ranges' and optionally 'groups', 'per_env', 'seed', got %r" % (cfg,))
+        if cfg['ranges'] is None:
+            raise ValueError('param_draw ranges must be a {key: (lo, hi)} dict or a list of one per agent slot')
+        try:
+            seed = int(cfg.get('seed', 0))
+        except (TypeError, ValueError):
+            raise ValueError('param_draw seed must be an int, got %r' % (cfg.get('seed'),))
+        d = pdraw.parse(cfg['ranges'], cfg.get('groups'), cfg.get('per_env', False), seed, num_agents)
+        pdraw.check_table(np.tile(hostmaps.params_vector(params), (1, num_agents, 1)), d)
+        return dict(cfg, seed=seed)
 
     def _autoreset_settings(self, cfg, batched, action_repeat):
         """autoreset kwarg -> {'poses': device table or list, 'max_episode_steps', 'seed', 'pose_gap', 'action_repeat'}, or

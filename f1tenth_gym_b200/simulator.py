@@ -22,6 +22,7 @@ import torch
 
 from . import _native as nat
 from . import maps as hostmaps
+from . import param_draw as pdraw
 
 
 RENDER_MAX_AGENTS = 64     # csrc/render.cuh F110_RENDER_MAX_AGENTS: car quads a block of k_render_views caches
@@ -427,6 +428,9 @@ class Simulator(object):
         self._episode_repeat = None
         self.ep_end_tick = self.ep_snap_rec = self.ep_snap_poses = self.ep_snap_wall_flag = None
         self.ep_scan_list = self.ep_scan_count = None
+        # per-episode parameter draws (C ABI f110_param_draw), set by set_param_draw; None: off
+        self._param_draw = self.param_draw = None
+        self.param_lo = self.param_hi = self.final_params = None
 
     # ------------------------------------------------------------------ configuration
     def set_map(self, map_path, map_ext, edt='scipy'):
@@ -471,11 +475,7 @@ class Simulator(object):
             else:
                 self.params_dev[agent_idx] = pv
             return
-        if not self.c.params_per_env:        # expand the shared table once
-            self.params_dev = self.params_dev.unsqueeze(0).repeat(N, 1, 1).contiguous()
-            self.c.params = nat.ptr(self.params_dev)
-            self.c.params_per_env = 1
-            self._graph = None
+        self._params_per_env()
         if per_env_values:
             pv = torch.as_tensor(params, dtype=torch.float64).to(self.device)
             pv = pv.reshape(N, -1, 18)                        # (N,1,18) broadcasts over agents, or (N,A,18)
@@ -486,6 +486,69 @@ class Simulator(object):
         tgt = self.params_dev if agent_idx < 0 else self.params_dev[:, agent_idx:agent_idx + 1]
         src = pv if (agent_idx < 0 or pv.shape[1] == 1) else pv[:, agent_idx:agent_idx + 1]
         tgt[m] = src.expand(N, tgt.shape[1], 18)[m]
+
+    def _params_per_env(self):
+        """Expand the shared parameter table to one row per env and slot ([N*A][18]), once."""
+        if not self.c.params_per_env:
+            self.params_dev = self.params_dev.unsqueeze(0).repeat(self.num_envs, 1, 1).contiguous()
+            self.c.params = nat.ptr(self.params_dev)
+            self.c.params_per_env = 1
+            self._graph = None
+
+    @property
+    def param_table(self):
+        """(N, A, 18) fp64 device view of the parameter table (maps.PARAM_KEYS order), the values the next tick runs with.  A
+        view of the live buffer: write through update_params, not into it."""
+        N, A = self.num_envs, self.num_agents
+        if self.c.params_per_env:
+            return self.params_dev.view(N, A, 18)
+        return self.params_dev.unsqueeze(0).expand(N, A, 18)
+
+    def set_param_draw(self, ranges, groups=None, per_env=False, seed=0):
+        """Per-episode dynamics randomisation (C ABI f110_param_draw, include/f110_param_draw.h): every env that starts a new
+        episode gets a fresh car, drawn on the device -- after the auto-reset of tick / autoreset / tick_repeat (after each tick
+        of the call), after the restart of episode mode, in every captured graph of those, and on redraw_params.  ranges: a
+        {key: (lo, hi)} dict for every slot, or a list of A such dicts ({} = the slot is never drawn); groups: lists of keys
+        that share one uniform number (e.g. [['m', 'I']]); per_env: every slot of an env shares its draws; seed: the draw's
+        seed.  The draw is f1tenth_gym_b200.param_draw.draw_rows.  Expands the table to per env as update_params does (one
+        host read checks its undrawn values) and drops a captured graph.  ValueError for what param_draw.parse refuses and for
+        undrawn values of a drawn slot that break the sign conditions (DESIGN §3.13).  None turns the draws off and keeps the
+        table."""
+        self._graph = None
+        if ranges is None:
+            self._param_draw = self.param_draw = None
+            self.param_lo = self.param_hi = self.final_params = None
+            return
+        d = pdraw.parse(ranges, groups, per_env, seed, self.num_agents)
+        pdraw.check_table(self.param_table.cpu().numpy(), d)
+        self._params_per_env()
+        dev = self.device
+        self.param_lo = torch.from_numpy(d['lo']).to(dev)
+        self.param_hi = torch.from_numpy(d['hi']).to(dev)
+        self.final_params = self.params_dev.clone()
+        keys = (C.c_uint32 * 32)(*[int(v) for v in d['keys']])
+        group = (C.c_int32 * 18)(*[int(v) for v in d['group']])
+        self._param_draw = nat.F110ParamDraw(nat.ptr(self.param_lo), nat.ptr(self.param_hi), keys, group,
+                                             1 if d['per_env'] else 0, d['seed'], nat.ptr(self.final_params))
+        self.param_draw = d         # the validated draw on the host (param_draw.parse), for draw_rows
+
+    def redraw_params(self, env_mask=None):
+        """Draw the masked envs' parameters now (None: every env), at the current tick counter (C ABI f110_params_draw), as
+        F110Env.reset does after placing the agents.  The draw is a function of (seed, tick counter, env, slot, group), so a
+        redraw at the counter of an env's previous draw repeats it.  ValueError without set_param_draw."""
+        if self._param_draw is None:
+            raise ValueError('redraw_params needs set_param_draw first')
+        m, mp = self._mask_ptr(env_mask)
+        nat.check(nat.lib().f110_params_draw(C.byref(self.c), C.byref(self._param_draw), mp, _stream_ptr(self.device)))
+
+    def _draw_autoreset(self, L):
+        if self._param_draw is not None:
+            nat.check(L.f110_params_draw_autoreset(C.byref(self.c), C.byref(self._param_draw), _stream_ptr(self.device)))
+
+    def _draw_episodes(self, L):
+        if self._param_draw is not None:
+            nat.check(L.f110_params_draw_episodes(C.byref(self.c), C.byref(self._param_draw), C.byref(self._episodes),
+                                                  _stream_ptr(self.device)))
 
     def set_noise(self, std_dev, seed=None):
         """Scan noise N(0, std_dev^2) (laser_models.py:429,450-452); 0 disables (parity runs)."""
@@ -597,22 +660,28 @@ class Simulator(object):
         """Reset every env whose ego collided to a hashed draw from start_poses (device (K,3) fp64, or a list of one
         (K_l,3) table per layer of a stacked map)."""
         table, n = self._start_table(start_poses)
-        nat.check(nat.lib().f110_autoreset_obst(C.byref(self.c), nat.ptr(table), n, pose_gap, int(seed), 0, self._obst_ref(),
-                                                _stream_ptr(self.device)))
+        L = nat.lib()
+        nat.check(L.f110_autoreset_obst(C.byref(self.c), nat.ptr(table), n, pose_gap, int(seed), 0, self._obst_ref(),
+                                        _stream_ptr(self.device)))
+        self._draw_autoreset(L)
 
     def tick(self, control_inputs, env_level=True, autoreset_poses=None, pose_gap=23, seed=12345):
         """One whole tick in three launches (C ABI f110_tick): step + lap logic + optional auto-reset, same
         results as step(); env_post_step(); autoreset()."""
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
+        L = nat.lib()
         if self._episode_path(table, env_level):
-            self._launch_episodes(nat.lib(), a, table, n, pose_gap, seed)
+            self._launch_episodes(L, a, table, n, pose_gap, seed)
+            self._draw_episodes(L)
             obs = self.observations()
             obs['terminated'], obs['truncated'] = self.ep_terminated, self.ep_truncated
             return obs
-        nat.check(nat.lib().f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                            C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
-                                            int(seed), self._obst_ref(), self._lidar_ref(), _stream_ptr(self.device)))
+        nat.check(L.f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                    C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
+                                    int(seed), self._obst_ref(), self._lidar_ref(), _stream_ptr(self.device)))
+        if table is not None:
+            self._draw_autoreset(L)
         return self.observations()
 
     # ------------------------------------------------------------------ episodes
@@ -697,7 +766,8 @@ class Simulator(object):
     @property
     def final_observation(self):
         """The last ended episode's final observation of each env, shaped like observations(): views of the final_* buffers,
-        bit for bit what the tick that ended it left, rewritten only when the env ends another episode."""
+        bit for bit what the tick that ended it left, rewritten only when the env ends another episode.  'params' (N, A, 18) is the
+        parameter table the episode ran with: with set_param_draw the rows the restart's draw replaced, else the table."""
         if self._episodes is None:
             return None
         N, A, B = self.num_envs, self.num_agents, self.num_beams
@@ -706,7 +776,8 @@ class Simulator(object):
                 'poses_x': st[0].view(N, A), 'poses_y': st[1].view(N, A), 'poses_theta': st[4].view(N, A),
                 'linear_vels_x': st[3].view(N, A), 'linear_vels_y': self._zeros_NA, 'ang_vels_z': st[5].view(N, A),
                 'collisions': self.final_collisions.view(N, A), 'collision_idx': self.final_collision_idx.view(N, A),
-                'lap_times': self.final_lap_times.view(N, A), 'lap_counts': self.final_lap_counts.view(N, A)}
+                'lap_times': self.final_lap_times.view(N, A), 'lap_counts': self.final_lap_counts.view(N, A),
+                'params': self.param_table if self._param_draw is None else self.final_params.view(N, A, 18)}
 
     def _episode_path(self, table, env_level):
         if self._episodes is None or table is None:
@@ -908,13 +979,21 @@ class Simulator(object):
         if episodes:
             self._episodes.track_seg = nat.ptr(self.track_seg)
             self._episode_repeat.track_delta_sum = nat.ptr(self.track_delta_sum) if progress else None
-        if not progress:
+        # the in-call auto-reset restarts envs on every tick: with a draw, each tick is issued alone and followed by the draw
+        per_tick_draw = self._param_draw is not None and not episodes and table is not None
+        if not progress and not per_tick_draw:
             ticks(0, K)
-            return
-        for t in range(K):
-            ticks(t, 1)
-            nat.check(L.f110_track_progress_sum(C.byref(self.c), C.byref(self.centerlines.c), C.byref(self._progress_c),
-                                                nat.ptr(self.track_delta_sum), 1 if t == 0 else 0, _stream_ptr(self.device)))
+        else:
+            for t in range(K):
+                ticks(t, 1)
+                if per_tick_draw:
+                    self._draw_autoreset(L)
+                if progress:
+                    nat.check(L.f110_track_progress_sum(C.byref(self.c), C.byref(self.centerlines.c), C.byref(self._progress_c),
+                                                        nat.ptr(self.track_delta_sum), 1 if t == 0 else 0,
+                                                        _stream_ptr(self.device)))
+        if episodes:
+            self._draw_episodes(L)
 
     def _repeat_call(self, env_level, progress):
         """The f110_repeat struct of a call (without the done outputs when the env level is off) after allocating what the
@@ -939,7 +1018,9 @@ class Simulator(object):
         is that tick's and done_any / done_tick count the ticks up to it; after the call it is restarted as tick() restarts it.
         The other envs are what tick_repeat leaves.  Adds 'terminated', 'truncated' and 'end_tick' (the tick 0..K-1 at which
         the episode ended, -1 = none); with progress=True a restarted env's track_delta_sum is 0.  Episode mode without
-        autoreset_poses raises ValueError."""
+        autoreset_poses raises ValueError.  With set_param_draw, an env restarted by the in-call auto-reset is drawn right after
+        its tick (the call is then issued tick by tick) and drives the rest of the call on its new car; in episode mode the
+        restarted envs are drawn after the call."""
         K = self._check_repeat(repeat)
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
@@ -1136,7 +1217,7 @@ class Simulator(object):
         repeat > 1 captures tick_repeat(actions, repeat) instead (done_any / done_tick with env_level); with progress=True the
         tracker is updated after every tick of the call and track_delta_sum (N*A,) holds the sum of the call's deltas.
         With episode mode set (set_episodes), autoreset_poses and env_level=True capture the episode tick instead, and with
-        repeat > 1 the episode call of tick_repeat."""
+        repeat > 1 the episode call of tick_repeat.  With set_param_draw the draws of those calls are captured with them."""
         assert actions.is_cuda and actions.dtype == torch.float64 and actions.is_contiguous()
         if progress and self.centerlines is None:
             raise ValueError('capture_graph(progress=True) needs set_centerlines first')
@@ -1154,7 +1235,7 @@ class Simulator(object):
                  'lidar_list_count', 'lidar_listed', 'ep_ticks', 'ep_terminated', 'ep_truncated', 'ep_length', 'final_state',
                  'final_scans', 'final_collisions', 'final_collision_idx', 'final_lap_times', 'final_lap_counts', 'ep_list',
                  'ep_list_count', 'ep_end_tick', 'ep_snap_rec', 'ep_snap_poses', 'ep_snap_wall_flag', 'ep_scan_list',
-                 'ep_scan_count')
+                 'ep_scan_count', 'params_dev', 'final_params')
         snapshot = {n: getattr(self, n).clone() for n in names if getattr(self, n, None) is not None}
         table, num_start = self._start_table(autoreset_poses)     # a list of per-layer tables is concatenated once, here
         episodes = self._episode_path(table, env_level)
@@ -1165,6 +1246,7 @@ class Simulator(object):
                 return
             if episodes:
                 self._launch_episodes(L, actions, table, num_start, pose_gap, autoreset_seed)
+                self._draw_episodes(L)
                 if progress:
                     self._launch_progress(L)
                 return
@@ -1172,6 +1254,8 @@ class Simulator(object):
                                         C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
                                         pose_gap, int(autoreset_seed), self._obst_ref(), self._lidar_ref(),
                                         _stream_ptr(self.device)))
+            if table is not None:
+                self._draw_autoreset(L)
             if progress:
                 self._launch_progress(L)
         side = torch.cuda.Stream(self.device)
@@ -1191,7 +1275,8 @@ class Simulator(object):
             ((call,) if K > 1 else ()) + ((self._obst, self.obstacle_boxes, self.obstacle_active, self.obstacle_hit) +
                                           self._obst_keep if self._obst is not None else ()) + \
             ((self._lidar, self.lidar_list, self.lidar_list_count, self.lidar_listed) if self._lidar is not None else ()) + \
-            ((self._episodes,) if episodes else ()) + ((self._episode_repeat,) if episodes and K > 1 else ())
+            ((self._episodes,) if episodes else ()) + ((self._episode_repeat,) if episodes and K > 1 else ()) + \
+            ((self.param_lo, self.param_hi, self.final_params) if self._param_draw is not None else ())
         return g
 
     def replay(self):
