@@ -822,20 +822,40 @@ __global__ void __launch_bounds__(MAXT, MINB) k_tail(f110_sim s, BeamView bv, in
 // per-agent SCALAR prologue (opponent vertices, six atan2, asin, sqrt, nearest-beam searches) that all 32 lanes of the agent's
 // warp execute redundantly.  Here a block owns EPB whole envs and works in three phases:
 //   1. one THREAD per (ego, opponent) pair does the scalar prologue -- 32 pairs per warp instead of one -- and leaves a task
-//      record in shared memory; one thread per agent also does the wall-hit zeroing, GJK and the collisions observation;
-//   2. one WARP per ego walks its tasks and ray-casts the windows beam-parallel (the same loop as finalize_agent);
+//      record in shared memory: the window and the beam intervals the cast visits; one thread per agent also does the wall-hit
+//      zeroing, GJK and the collisions observation;
+//   2. the beams of all tasks of one opponent rank form one flat list, and every thread of the block casts its share of it
+//      (below); one pass per rank;
 //   3. one thread per env: lap logic + auto-reset (as in k_tail).
-struct TailTask {
+// A task visits 33-56 beams on the benchmark's poses (tools/tail_cast_study.py), so a warp per ego -- the first version of
+// phase 2 -- ran 2-3 loop iterations per opponent, each a serial chain of a scan load (mostly DRAM: the march's scans
+// outgrow L2), an fp64 sincos and four edge tests, for ~10 egos one after the other per warp at cfg3.  The flat list spreads
+// the same beams over every thread at once.
+// The TailTask records of k_lidar_cast / k_episode_cast are separate: changing them would change those kernels.
+#define F110_TAIL2_IVALS 4               // beam intervals per task (fov <= 2 pi, cone <= pi/2 + 0.05: at most 4)
+struct Tail2Task {                       // 120 bytes, as the TailTask it replaced: the launch record's smem is unchanged
+    double phi, cone;
+    double v[8];
+    int iv[2 * F110_TAIL2_IVALS];        // disjoint beam intervals [iv[2q], iv[2q + 1]], ascending
+    int pad[2];
+};
+struct TailTask {                        // the records of k_lidar_cast / k_episode_cast (warp per ego)
     double px, py, yaw, phi, cone;
     double v[8];
     int lo, hi, active, pad;
 };
 #define F110_TAIL2_THREADS 256
+#define F110_TAIL2_MAX_AGENTS 128        // agents per block: f110_debug_set_tail2 caps forced shapes here
+
+// dynamic shared memory of k_tail2 for epb envs of A agents: the task records
+static inline size_t tail2_smem_bytes(int epb, int A) { return (size_t)epb * A * (A - 1) * sizeof(Tail2Task); }
 
 __global__ void __launch_bounds__(F110_TAIL2_THREADS, 3) k_tail2(f110_sim s, BeamView bv, int env_level, AutoResetArgs ar,
                                                                   double max_scan_range, int envs_per_block) {
     extern __shared__ __align__(16) unsigned char tail2_smem[];
-    TailTask *tasks = reinterpret_cast<TailTask *>(tail2_smem);
+    Tail2Task *tasks = reinterpret_cast<Tail2Task *>(tail2_smem);
+    __shared__ double ego_pose[3][F110_TAIL2_MAX_AGENTS];      // px, py and the yaw the cast uses, per ego
+    __shared__ int offs[3 * (F110_TAIL2_MAX_AGENTS + 1)];      // per opponent rank: beams per ego, then their exclusive scan
     const int A = s.num_agents, NA = s.num_envs * A;
     const int opp = A - 1;                                    // tasks per agent
     const int env0 = blockIdx.x * envs_per_block;
@@ -858,6 +878,7 @@ __global__ void __launch_bounds__(F110_TAIL2_THREADS, 3) k_tail2(f110_sim s, Bea
         const double cyaw = hit ? 1.0 : pa[3], syaw = hit ? 0.0 : pa[4];
         const double *pb = s.agent_poses + 5 * (size_t)(env * A + j);
         if (oj == 0) {
+            ego_pose[0][la] = px; ego_pose[1][la] = py; ego_pose[2][la] = yaw;
             // per-agent duties: wall-hit zeroing, GJK against the other agents (collision_multiple :184-212), collisions obs
             if (hit) {
 #pragma unroll
@@ -880,16 +901,14 @@ __global__ void __launch_bounds__(F110_TAIL2_THREADS, 3) k_tail2(f110_sim s, Bea
             s.collision_idx[a] = cidx;
         }
         // ray_cast_agents (:206-227): the scalar part of one opponent
-        TailTask &k = tasks[t];
+        Tail2Task &k = tasks[t];
         const double *p = s.params + (size_t)(s.params_per_env ? a : slot) * F110_NPARAM;
         const double length = p[P_LENGTH], width = p[P_WIDTH];
         const double half_diag = 0.5 * sqrt(length * length + width * width);
         const double ddx = pb[0] - px, ddy = pb[1] - py;
         const double far = max_scan_range + half_diag;
-        int active = 1;
-        if (ddx * ddx + ddy * ddy > far * far) active = 0;     // cannot shorten any beam (see finalize_agent)
-        k.active = active;
-        if (active) {
+        int n = 0;
+        if (ddx * ddx + ddy * ddy <= far * far) {              // else it cannot shorten any beam (see finalize_agent)
             double v[8];
             get_vertices_cs(pb[0], pb[1], pb[3], pb[4], length, width, v);
             int lo, hi;
@@ -901,70 +920,120 @@ __global__ void __launch_bounds__(F110_TAIL2_THREADS, 3) k_tail2(f110_sim s, Bea
                 const double dist = sqrt(ddx * ddx + ddy * ddy);
                 if (dist > 1.25 * half_diag) cone = asin(half_diag / dist) + 0.05;
             }
-            k.px = px; k.py = py; k.yaw = yaw; k.phi = phi; k.cone = cone; k.lo = lo; k.hi = hi;
+            k.phi = phi; k.cone = cone;
 #pragma unroll
             for (int q = 0; q < 8; q++) k.v[q] = v[q];
-        }
-    }
-    __syncthreads();
-
-    // ---- phase 2: warp per ego, its opponents one after the other (they update the same scan)
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    for (int la = warp; la < agents_here; la += nwarps) {
-        const int a = env0 * A + la;
-        float *scan = s.scans + (size_t)a * bv.num_beams;
-        for (int oj = 0; oj < opp; oj++) {
-            const TailTask &k = tasks[la * opp + oj];
-            if (!k.active) continue;
-            const double px = k.px, py = k.py, yaw = k.yaw, phi = k.phi, cone = k.cone;
-            const int lo = k.lo, hi = k.hi;
-            double v[8];
-#pragma unroll
-            for (int q = 0; q < 8; q++) v[q] = k.v[q];
-            auto cast_beams = [&](int i0, int i1) {
-                for (int i = i0 + lane; i <= i1; i += 32) {
-                    const float cur = scan[i];
-                    double bt = yaw + bv.scan_angles[i];
-                    double dl = bt - phi;
-                    dl = dl - (2 * M_PI) * rint(dl * (1.0 / (2 * M_PI)));
-                    const double adl = fabs(dl);
-                    if (adl > cone && (M_PI - adl) > cone) continue;
-                    double v3x, v3y;
-                    sincos(bt + M_PI / 2., &v3y, &v3x);
-                    const double curd = (double)cur;
-                    double r = INFINITY;
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        int e2 = (e + 1) & 3;
-                        double d = get_range_below(px, py, v3x, v3y, v[2 * e], v[2 * e + 1], v[2 * e2], v[2 * e2 + 1], curd);
-                        if (d < r) r = d;
-                    }
-                    float rf = (float)r;
-                    if (rf < cur) scan[i] = rf;
-                }
-            };
+            // the beams to visit: [lo, hi], or in a wide window the intervals around the centres (phi - yaw) + m pi (see
+            // finalize_agent).  Clipping each interval to start after the previous one is exact: centres are pi apart and
+            // cone < pi/2 here, so they do not overlap anyway, and a second visit of a beam by the same opponent stores nothing.
+            int nq = 0;
+            bool whole = true;
             if (cone < 3.5 && hi - lo >= 96) {
-                const double base = wrap_2pi_diff(phi - yaw), half = bv.fov / 2., inv_inc = 1.0 / bv.angle_increment;   // (see finalize_agent)
+                whole = false;
+                const double base = wrap_2pi_diff(phi - yaw), half = bv.fov / 2., inv_inc = 1.0 / bv.angle_increment;
                 const int m0 = max(-3, (int)floor((-half - cone - 0.02 - base) * (1.0 / M_PI))),
                           m1 = min(5, (int)ceil((half + cone + 0.02 - base) * (1.0 / M_PI)));
+                int next = lo;
                 for (int m = m0; m <= m1; m++) {
                     const double c = base + (double)m * M_PI;
                     const double f0 = (c - cone + half) * inv_inc - 2.0, f1 = (c + cone + half) * inv_inc + 2.0;
                     if (f1 < (double)lo || f0 > (double)hi) continue;
-                    const int i0 = max(lo, (int)floor(fmax(f0, (double)lo))), i1 = min(hi, (int)ceil(fmin(f1, (double)hi)));
-                    cast_beams(i0, i1);
+                    const int i0 = max(next, (int)floor(fmax(f0, (double)lo))), i1 = min(hi, (int)ceil(fmin(f1, (double)hi)));
+                    if (i0 > i1) continue;
+                    // more intervals than the record holds (fov > 2 pi, or a cone the window rule cannot make): [lo, hi]
+                    // instead, which is exact -- the per-beam cone test decides
+                    if (nq == F110_TAIL2_IVALS) { whole = true; break; }
+                    k.iv[2 * nq] = i0; k.iv[2 * nq + 1] = i1;
+                    n += i1 - i0 + 1;
+                    nq++;
+                    next = i1 + 1;
                 }
-            } else {
-                cast_beams(lo, hi);
             }
-            __syncwarp();
+            if (whole) { k.iv[0] = lo; k.iv[1] = hi; n = hi - lo + 1; nq = 1; }
+        }
+        offs[oj * (agents_here + 1) + la] = n;                  // beams the task visits (0: none)
+    }
+    __syncthreads();
+
+    // ---- phase 2a: exclusive scan of the tasks' beam counts, one array per opponent rank (a warp per rank)
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    for (int oj = warp; oj < opp; oj += nwarps) {
+        int *o = offs + oj * (agents_here + 1);
+        int run = 0;
+        for (int l0 = 0; l0 < agents_here; l0 += 32) {
+            const int la = l0 + lane;
+            const int n = la < agents_here ? o[la] : 0;
+            int incl = n;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const int u = __shfl_up_sync(0xffffffffu, incl, d);
+                if (lane >= d) incl += u;
+            }
+            if (la < agents_here) o[la] = run + incl - n;
+            run += __shfl_sync(0xffffffffu, incl, 31);
+        }
+        if (lane == 0) o[agents_here] = run;
+    }
+    __syncthreads();
+
+    // ---- phase 2b: flat beam list of each opponent rank over the whole block.  Flat index f of rank oj is beam f - o[la] of
+    // ego la's intervals, o[la] <= f < o[la + 1]; thread tid takes f = tid, tid + blockDim, ...  Within a pass an (ego, beam)
+    // pair occurs once, so no two threads touch one scan entry; the passes run in rank order, so a beam that two opponents
+    // shorten sees them in k_tail's order.  Per beam the statements are finalize_agent's, except that the cone test comes
+    // before the scan load (a rejected beam loads nothing).  Measured on the H100 at cfg3 (16384 x 2), k_tail2: 34 us with
+    // one beam at a time per thread, 39.5 us when a thread first issued the loads of a batch of 4 beams, and no gain from an
+    // L2 prefetch of the tasks' scan lines in phase 1 (39.4 us with, 39.3 without, at the batch of 4).
+    const int B = bv.num_beams;
+    float *scans0 = s.scans + (size_t)env0 * A * B;
+    for (int oj = 0; oj < opp; oj++) {
+        if (oj) __syncthreads();
+        const int *o = offs + oj * (agents_here + 1);
+        const int total = o[agents_here];
+        int la = 0;
+        if ((int)threadIdx.x < total) {                       // the task of the first index: largest la with o[la] <= tid
+            int hi = agents_here;
+            while (hi - la > 1) {
+                const int mid = (la + hi) >> 1;
+                if (o[mid] <= (int)threadIdx.x) la = mid;
+                else hi = mid;
+            }
+        }
+        for (int f = threadIdx.x; f < total; f += blockDim.x) {
+            while (o[la + 1] <= f) la++;
+            const Tail2Task &k = tasks[la * opp + oj];
+            int r = f - o[la], q = 0;
+            while (r > k.iv[2 * q + 1] - k.iv[2 * q]) { r -= k.iv[2 * q + 1] - k.iv[2 * q] + 1; q++; }
+            const int i = k.iv[2 * q] + r;
+            double bt = ego_pose[2][la] + bv.scan_angles[i];
+            double dl = bt - k.phi;
+            dl = dl - (2 * M_PI) * rint(dl * (1.0 / (2 * M_PI)));
+            const double adl = fabs(dl);
+            if (adl > k.cone && (M_PI - adl) > k.cone) continue;
+            float *scan = scans0 + (size_t)la * B;
+            const float cur = scan[i];
+            const double px = ego_pose[0][la], py = ego_pose[1][la];
+            double v[8];
+#pragma unroll
+            for (int e = 0; e < 8; e++) v[e] = k.v[e];
+            double v3x, v3y;
+            sincos(bt + M_PI / 2., &v3y, &v3x);
+            const double curd = (double)cur;
+            double rr = INFINITY;
+#pragma unroll
+            for (int e = 0; e < 4; e++) {
+                int e2 = (e + 1) & 3;
+                double d = get_range_below(px, py, v3x, v3y, v[2 * e], v[2 * e + 1], v[2 * e2], v[2 * e2 + 1], curd);
+                if (d < rr) rr = d;
+            }
+            float rf = (float)rr;
+            if (rf < cur) scan[i] = rf;
         }
     }
     __syncthreads();
 
-    // ---- phase 3: env level
-    if ((int)threadIdx.x < envs_here) {
-        const int env = env0 + (int)threadIdx.x;
+    // ---- phase 3: env level (a loop: a forced shape of f110_debug_set_tail2 may have more envs than threads)
+    for (int e = threadIdx.x; e < envs_here; e += blockDim.x) {
+        const int env = env0 + e;
         if (env_level) env_post_step_one(s, env);
         if (ar.start_poses) autoreset_one(s, env, ar);
     }
@@ -2072,9 +2141,13 @@ static int launch_tail(const f110_sim *sim, const f110_map *map, const BeamView 
             // leaves the GPU two-thirds empty for the second half of the kernel, and grids of whole waves measured about a quarter
             // faster.  So: 128-thread blocks of up to 47 agents, and as many envs per block as fill a whole number of waves
             // (the wave size comes from the occupancy query and the SM count, not from a fixed device).
+            // Re-swept with the flat phase 2 (every thread casts), k_tail2 in us on an H100 80GB HBM3 at 700 W, threads:agents:
+            //   cfg3 (16384 x 2):  this rule (128:42, one wave) 32.8, 256:42 33.3, 256:96 35.8, 128:24 40.8, 256:16 46.6, 128:12 54.2
+            //   cfg2x2 (4096 x 2): this rule (128:12) 19.8 (forced to the same shape 20.1), 256:16 21.4, 128:24 23.8, 256:42 28.1
+            // so the rule stands.
             static int per_sm = 0;                          // resident 128-thread blocks per SM
             if (per_sm == 0) {
-                const size_t sm0 = (size_t)(47 / sim->num_agents) * sim->num_agents * (sim->num_agents - 1) * sizeof(TailTask);
+                const size_t sm0 = tail2_smem_bytes(47 / sim->num_agents, sim->num_agents);
                 if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_tail2, 128, sm0) != cudaSuccess || per_sm < 1) { per_sm = -1; cudaGetLastError(); }
             }
             if (per_sm > 0) {
@@ -2086,7 +2159,9 @@ static int launch_tail(const f110_sim *sim, const f110_map *map, const BeamView 
             }
         }
         ts.kernel = TailShape::TAIL2; ts.epb = epb; ts.threads = t2; ts.grid = (sim->num_envs + epb - 1) / epb;
-        ts.smem = (size_t)epb * sim->num_agents * (sim->num_agents - 1) * sizeof(TailTask);
+        ts.smem = tail2_smem_bytes(epb, sim->num_agents);
+        if (ts.smem > 40 * 1024)   // with the ~4.6 KB of static arrays past the 48 KB default: forced shapes of A = 4 only
+            cudaFuncSetAttribute(k_tail2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ts.smem);
         launch_k(k_tail2, dim3(ts.grid), dim3(t2), ts.smem, st, pdl, *sim, bv, fused ? (int)tail->env_level : 0,
                  fused ? tail->ar : no_ar, max_scan, epb);
         LAUNCH_CHECK("k_tail2");
