@@ -2323,24 +2323,56 @@ static bool ttc_path_ok(const f110_sim *sim, const f110_map *map, const f110_bea
     return sim->noise_std == 0.0 && m.lean && lean_family && sim->march_rec && map->sincos2 && map->dt_min_positive > map->eps &&
            beams->side_max > 0.0 && beams->side_max < map->max_range && sim->num_agents <= 32;
 }
-template <int UNITS>
-static int ttc_grid(bool count, unsigned *grid) {
-    static int per_sm[2] = {0, 0};
-    int &n = per_sm[count ? 1 : 0];
-    if (n <= 0) {
-        if (count) CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, true>, F110_TTC_THREADS, 0));
-        else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_march_ttc<UNITS, false>, F110_TTC_THREADS, 0));
-        if (n <= 0) return F110_ERR_INVALID;
+// The units (F110_SCAN_UNITS_*) k_march_ttc and k_restart_march run in for a march plan.  They follow the family, never the
+// queue length, so a tick's plan and its lidar-mask plan agree.
+static int scan_units(const MarchPlan &m) {
+    return m.rot ? F110_SCAN_UNITS_ROT : m.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+}
+// The UNITS build of a kernel: f(units) with the run-time F110_SCAN_UNITS_* value as a std::integral_constant.
+template <typename F>
+static void dispatch_units(int units, F &&f) {
+    if (units == F110_SCAN_UNITS_ROT) f(std::integral_constant<int, F110_SCAN_UNITS_ROT>());
+    else if (units == F110_SCAN_UNITS_CELLS) f(std::integral_constant<int, F110_SCAN_UNITS_CELLS>());
+    else f(std::integral_constant<int, F110_SCAN_UNITS_METRES>());
+}
+static void launch_march_ttc(const TtcK &q, int units, bool count, unsigned grid, cudaStream_t st) {
+    dispatch_units(units, [&](auto u) {
+        if (count) k_march_ttc<decltype(u)::value, true><<<grid, F110_TTC_THREADS, 0, st>>>(q);
+        else k_march_ttc<decltype(u)::value, false><<<grid, F110_TTC_THREADS, 0, st>>>(q);
+    });
+}
+static void launch_restart_march(const TtcK &q, const RestartK &r, int units, bool count, unsigned grid, cudaStream_t st) {
+    dispatch_units(units, [&](auto u) {
+        if (count) k_restart_march<decltype(u)::value, true><<<grid, F110_TTC_THREADS, 0, st>>>(q, r);
+        else k_restart_march<decltype(u)::value, false><<<grid, F110_TTC_THREADS, 0, st>>>(q, r);
+    });
+}
+// The fixed grid of a grid-stride kernel of F110_TTC_THREADS threads: resident blocks per SM x SMs, the occupancy of each
+// kernel instance queried once.
+template <auto KERNEL>
+static int resident_grid(unsigned *grid) {
+    static int per_sm = 0;
+    if (per_sm <= 0) {
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, KERNEL, F110_TTC_THREADS, 0));
+        if (per_sm <= 0) return F110_ERR_INVALID;
     }
-    *grid = (unsigned)n * (unsigned)num_sms();
+    *grid = (unsigned)per_sm * (unsigned)num_sms();
     return F110_OK;
 }
-// k_march_ttc's units (F110_SCAN_UNITS_*) for the tick's march, and its fixed grid: resident blocks per SM x SMs
+// the grid of k_march_ttc, or with restart of k_restart_march
+static int ttc_grid(bool restart, int units, bool count, unsigned *grid) {
+    int rc = F110_OK;
+    dispatch_units(units, [&](auto u) {
+        constexpr int U = decltype(u)::value;
+        if (restart) rc = count ? resident_grid<k_restart_march<U, true>>(grid) : resident_grid<k_restart_march<U, false>>(grid);
+        else rc = count ? resident_grid<k_march_ttc<U, true>>(grid) : resident_grid<k_march_ttc<U, false>>(grid);
+    });
+    return rc;
+}
+// k_march_ttc's units for the tick's march, and its grid
 static int plan_ttc(const MarchPlan &m, int *units, unsigned *grid) {
-    *units = m.rot ? F110_SCAN_UNITS_ROT : m.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
-    return *units == F110_SCAN_UNITS_ROT ? ttc_grid<F110_SCAN_UNITS_ROT>(m.count, grid)
-         : *units == F110_SCAN_UNITS_CELLS ? ttc_grid<F110_SCAN_UNITS_CELLS>(m.count, grid)
-                                           : ttc_grid<F110_SCAN_UNITS_METRES>(m.count, grid);
+    *units = scan_units(m);
+    return ttc_grid(false, *units, m.count, grid);
 }
 
 struct TickPlan {
@@ -2432,11 +2464,20 @@ static int plan_repeat(const f110_sim *sim, const f110_map *map, const f110_marc
     if ((rc = plan_tick(sim, map, tables, beams, actions, &rp->tick))) return rc;
     const MarchPlan &m = rp->tick.march;
     rp->ttc = repeat > 1 && ttc_path_ok(sim, map, beams, m);
-    rp->units = m.rot ? F110_SCAN_UNITS_ROT : m.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+    rp->units = scan_units(m);
     rp->grid = 0u;
     if (!rp->ttc) return F110_OK;
     return plan_ttc(m, &rp->units, &rp->grid);
 }
+// the tail options and plans of a held-action call (f110_tick_repeat_ticks_lidar, f110_tick_repeat_episodes_ticks)
+struct RepeatCall {
+    TailOpts t;
+    RepeatPlan rp;
+    TickPlan last;           // with a lidar mask: the last tick of the call, the plain tick's plan with the mask
+    ObstPlan ob;
+    bool masked;
+    TickPlan &last_tick() { return masked ? last : rp.tick; }
+};
 
 // list / count: the agents k_ttc_select listed
 static TtcK fill_ttc_k(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const TickPlan &tp, const uint32_t *list,
@@ -2472,32 +2513,29 @@ static TtcK fill_ttc_k(const f110_sim *sim, const f110_map *map, const f110_beam
     return q;
 }
 
-template <int UNITS>
-static void launch_march_ttc_t(const TtcK &q, bool count, unsigned grid, cudaStream_t st) {
-    if (count) k_march_ttc<UNITS, true><<<grid, F110_TTC_THREADS, 0, st>>>(q);
-    else k_march_ttc<UNITS, false><<<grid, F110_TTC_THREADS, 0, st>>>(q);
-}
-static void launch_march_ttc(const TtcK &q, int units, bool count, unsigned grid, cudaStream_t st) {
-    if (units == F110_SCAN_UNITS_ROT) launch_march_ttc_t<F110_SCAN_UNITS_ROT>(q, count, grid, st);
-    else if (units == F110_SCAN_UNITS_CELLS) launch_march_ttc_t<F110_SCAN_UNITS_CELLS>(q, count, grid, st);
-    else launch_march_ttc_t<F110_SCAN_UNITS_METRES>(q, count, grid, st);
+// k_ttc_select: the agents a wall could stop into list / count, except those of the slots in `skip`
+static int launch_ttc_select(const f110_sim *sim, const f110_map *map, const MarchPlan &m, uint32_t *list, uint32_t *count,
+                             unsigned long long *marched, uint32_t skip, cudaStream_t st) {
+    const int NA = sim->num_envs * sim->num_agents;
+    TtcSelectK sel;
+    sel.rec = reinterpret_cast<const double2 *>(sim->march_rec); sel.list = list; sel.count = count;
+    sel.marched = marched; sel.d0_scale = m.cell_units ? map->resolution : 1.0; sel.max_range = map->max_range;
+    sel.agents = (unsigned)NA; sel.skip = skip; sel.num_agents = (unsigned)sim->num_agents;
+    k_ttc_select<<<(NA + F110_TTC_SELECT_THREADS - 1) / F110_TTC_SELECT_THREADS, F110_TTC_SELECT_THREADS, 0, st>>>(sel);
+    LAUNCH_CHECK("k_ttc_select");
+    return F110_OK;
 }
 
 // one intermediate tick of the short path
 static int launch_ttc_tick(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions,
                            const RepeatPlan &rp, const f110_repeat *rep, int tick, const TailOpts &tail, cudaStream_t st) {
+    int rc;
     const MarchPlan &m = rp.tick.march;
-    const int NA = sim->num_envs * sim->num_agents;
     // k_dynamics without its queue-building blocks: the queue is built once, by the last tick of the call
     k_dynamics<<<m.dyn_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, m.dyn_blocks,
                                              fill_first_lookup(sim, map, beams, rp.tick.geom, m));
     LAUNCH_CHECK("k_dynamics");
-    TtcSelectK sel;
-    sel.rec = reinterpret_cast<const double2 *>(sim->march_rec); sel.list = rep->list; sel.count = rep->list_count + tick;
-    sel.marched = rep->marched_agents; sel.d0_scale = m.cell_units ? map->resolution : 1.0; sel.max_range = map->max_range;
-    sel.agents = (unsigned)NA; sel.skip = 0u; sel.num_agents = (unsigned)sim->num_agents;
-    k_ttc_select<<<(NA + F110_TTC_SELECT_THREADS - 1) / F110_TTC_SELECT_THREADS, F110_TTC_SELECT_THREADS, 0, st>>>(sel);
-    LAUNCH_CHECK("k_ttc_select");
+    if ((rc = launch_ttc_select(sim, map, m, rep->list, rep->list_count + tick, rep->marched_agents, 0u, st))) return rc;
     launch_march_ttc(fill_ttc_k(sim, map, beams, rp.tick, rep->list, rep->list_count + tick), rp.units, m.count, rp.grid, st);
     LAUNCH_CHECK("k_march_ttc");
     const int epb = std::max(1, F110_TAIL_NOSCAN_THREADS / sim->num_agents);
@@ -2531,7 +2569,6 @@ static int launch_lidar_tick(const f110_sim *sim, const f110_map *map, const f11
     MarchPlan &plan = tp.march;
     const f110_lidar &ld = *tp.lidar;
     const unsigned S = tp.lidar_slots;
-    const int NA = sim->num_envs * sim->num_agents;
     const LidarOrder lo = {ld.mask, S};
     k_dynamics<<<plan.dyn_blocks, 128, 0, st>>>(*sim, actions, beams->fov, (double)map->theta_dis, plan.dyn_blocks,
                                                 fill_first_lookup(sim, map, beams, tp.geom, plan));
@@ -2542,12 +2579,7 @@ static int launch_lidar_tick(const f110_sim *sim, const f110_map *map, const f11
     }
     if (S && (rc = launch_march_plan(plan, sim, map, tables, beams, tp.geom, false, st))) return rc;
     CUDA_TRY(cudaMemsetAsync(ld.list_count, 0, sizeof(uint32_t), st));
-    TtcSelectK sel;
-    sel.rec = reinterpret_cast<const double2 *>(sim->march_rec); sel.list = ld.list; sel.count = ld.list_count;
-    sel.marched = ld.listed; sel.d0_scale = plan.cell_units ? map->resolution : 1.0; sel.max_range = map->max_range;
-    sel.agents = (unsigned)NA; sel.skip = ld.mask; sel.num_agents = (unsigned)sim->num_agents;
-    k_ttc_select<<<(NA + F110_TTC_SELECT_THREADS - 1) / F110_TTC_SELECT_THREADS, F110_TTC_SELECT_THREADS, 0, st>>>(sel);
-    LAUNCH_CHECK("k_ttc_select");
+    if ((rc = launch_ttc_select(sim, map, plan, ld.list, ld.list_count, ld.listed, ld.mask, st))) return rc;
     launch_march_ttc(fill_ttc_k(sim, map, beams, tp, ld.list, ld.list_count), tp.ttc_units, plan.count, tp.ttc_grid, st);
     LAUNCH_CHECK("k_march_ttc");
     const BeamView bv = make_view(beams);
@@ -2600,22 +2632,55 @@ static bool episode_march_ok(const MarchPlan &m) {
     return m.lean && (m.family == MarchFamily::LEAN || m.family == MarchFamily::LEAN_BRICK || m.family == MarchFamily::LEAN_HET ||
                       m.family == MarchFamily::LEAN_HET_RES || m.family == MarchFamily::LEAN_ROT);
 }
-template <int UNITS>
-static int restart_grid(bool count, unsigned *grid) {
-    static int per_sm[2] = {0, 0};
-    int &n = per_sm[count ? 1 : 0];
-    if (n <= 0) {
-        if (count) CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_restart_march<UNITS, true>, F110_TTC_THREADS, 0));
-        else CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, k_restart_march<UNITS, false>, F110_TTC_THREADS, 0));
-        if (n <= 0) return F110_ERR_INVALID;
+// The scans of the envs on r.list / r.count for the slots in r.lidar, from the plan tp, on `grid` blocks of k_restart_march.
+// restart, the kernel that listed the ended envs (k_episode_end / k_episode_restart): their restart on view = *sim --
+//   k_episode_dyn, k_restart_march, k_episode_cast, k_episode_tail, k_episode_obstacles -- and the `episodes restart=` record.
+// restart NULL: the final-scan pass on a snapshot `view` whose march records are `rec` -- k_restart_march without the lookup
+//   count, k_episode_cast, and k_episode_obstacles without box contact (ObstK.hit NULL); the caller writes its record.
+static int launch_restart(const char *restart, const f110_sim &view, const double *rec, const f110_map *map,
+                          const f110_beams *beams, const TickPlan &tp, const RestartK &r, unsigned grid, cudaStream_t st) {
+    const int N = view.num_envs, A = view.num_agents, NA = N * A;
+    if (restart) {
+        k_episode_dyn<<<(NA + 127) / 128, 128, 0, st>>>(view, beams->fov, (double)map->theta_dis,
+                                                        fill_first_lookup(&view, map, beams, tp.geom, tp.march), r.list, r.count);
+        LAUNCH_CHECK("k_episode_dyn");
     }
-    *grid = (unsigned)n * (unsigned)num_sms();
+    TtcK q = fill_ttc_k(&view, map, beams, tp, r.list, r.count);
+    q.rec = reinterpret_cast<const double2 *>(rec);
+    launch_restart_march(q, r, scan_units(tp.march), restart && tp.march.count, grid, st);
+    LAUNCH_CHECK("k_restart_march");
+    const BeamView bv = make_view(beams);
+    const double max_scan = max_scan_range(&view, map);
+    const unsigned slots = (unsigned)__builtin_popcount(r.lidar);
+    if (A > 1 && slots) {
+        const LidarOrder lo = {r.lidar, slots};
+        k_episode_cast<<<(unsigned)(((unsigned long long)N * slots + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS),
+                         32 * F110_LIDAR_CAST_WARPS, 0, st>>>(view, bv, lo, r.list, r.count, max_scan);
+        LAUNCH_CHECK("k_episode_cast");
+    }
+    if (restart) {
+        k_episode_tail<<<(N + 127) / 128, 128, 0, st>>>(view, r.list, r.count);
+        LAUNCH_CHECK("k_episode_tail");
+    }
+    if (tp.obst) {
+        ObstK o = tp.obst->k;
+        o.lidar = r.lidar;
+        if (!restart) o.hit = nullptr;
+        k_episode_obstacles<<<(unsigned)(((long long)NA * 32 + 127) / 128), 128, 0, st>>>(view, bv, o, max_scan, r.list, r.count);
+        LAUNCH_CHECK("k_episode_obstacles");
+    }
+    if (restart)
+        append_launch_record(" episodes restart=%s+k_episode_dyn+k_restart_march%s+k_episode_tail%s restart_grid=%u", restart,
+                             (A > 1 && slots) ? "+k_episode_cast" : "", tp.obst ? "+k_episode_obstacles" : "", grid);
     return F110_OK;
 }
-template <int UNITS>
-static void launch_restart_march_t(const TtcK &q, const RestartK &r, bool count, unsigned grid, cudaStream_t st) {
-    if (count) k_restart_march<UNITS, true><<<grid, F110_TTC_THREADS, 0, st>>>(q, r);
-    else k_restart_march<UNITS, false><<<grid, F110_TTC_THREADS, 0, st>>>(q, r);
+static EpisodeK episode_k(const f110_episodes *ep) {
+    EpisodeK k;
+    k.ticks = ep->ticks; k.length = ep->length; k.terminated = ep->terminated; k.truncated = ep->truncated;
+    k.final_state = ep->final_state; k.final_collisions = ep->final_collisions; k.final_lap_times = ep->final_lap_times;
+    k.final_lap_counts = ep->final_lap_counts; k.final_collision_idx = ep->final_collision_idx;
+    k.list = ep->list; k.count = ep->list_count; k.track_seg = ep->track_seg; k.max_ticks = ep->max_ticks;
+    return k;
 }
 static int check_episodes(const f110_sim *sim, const f110_episodes *ep, const double *start_poses) {
     if (!ep || !start_poses) return F110_ERR_INVALID;
@@ -2896,61 +2961,88 @@ int f110_tick_episodes(const f110_sim *sim, const f110_map *map, const f110_marc
         if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
         tp.obst = &ob;
     }
-    const int units = tp.march.rot ? F110_SCAN_UNITS_ROT : tp.march.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
     unsigned grid = 0u;
-    if ((rc = units == F110_SCAN_UNITS_ROT ? restart_grid<F110_SCAN_UNITS_ROT>(tp.march.count, &grid)
-            : units == F110_SCAN_UNITS_CELLS ? restart_grid<F110_SCAN_UNITS_CELLS>(tp.march.count, &grid)
-                                             : restart_grid<F110_SCAN_UNITS_METRES>(tp.march.count, &grid)))
-        return rc;
+    if ((rc = ttc_grid(true, scan_units(tp.march), tp.march.count, &grid))) return rc;
 
     if ((rc = launch_tick(sim, map, tables, beams, actions, tp, st, nullptr, &t))) return rc;
-    const int N = sim->num_envs, A = sim->num_agents, NA = N * A;
+    const int N = sim->num_envs, A = sim->num_agents;
     const uint32_t all = A == 32 ? 0xFFFFFFFFu : (1u << A) - 1u;
     // the slots whose scans exist: the mask on the short path, every slot when the tick ignores it (or has none)
     const uint32_t scan_slots = tp.lidar ? tp.lidar->mask : all;
     const uint32_t final_slots = (lidar && lidar->mask != F110_LIDAR_ALL) ? (lidar->mask & all) : all;
-    EpisodeK k;
-    k.ticks = ep->ticks; k.length = ep->length; k.terminated = ep->terminated; k.truncated = ep->truncated;
-    k.final_state = ep->final_state; k.final_collisions = ep->final_collisions; k.final_lap_times = ep->final_lap_times;
-    k.final_lap_counts = ep->final_lap_counts; k.final_collision_idx = ep->final_collision_idx;
-    k.list = ep->list; k.count = ep->list_count; k.track_seg = ep->track_seg; k.max_ticks = ep->max_ticks;
     ObstDraw no_draw;
     memset(&no_draw, 0, sizeof(no_draw));
     CUDA_TRY(cudaMemsetAsync(ep->list_count, 0, sizeof(uint32_t), st));
-    k_episode_end<<<(N + 127) / 128, 128, 0, st>>>(*sim, ar, k, obst ? ob.d : no_draw);
+    k_episode_end<<<(N + 127) / 128, 128, 0, st>>>(*sim, ar, episode_k(ep), obst ? ob.d : no_draw);
     LAUNCH_CHECK("k_episode_end");
-    k_episode_dyn<<<(NA + 127) / 128, 128, 0, st>>>(*sim, beams->fov, (double)map->theta_dis,
-                                                    fill_first_lookup(sim, map, beams, tp.geom, tp.march), ep->list, ep->list_count);
-    LAUNCH_CHECK("k_episode_dyn");
     RestartK r;
     r.list = ep->list; r.count = ep->list_count; r.scans = sim->scans; r.final_scans = ep->final_scans;
     r.tick_counter = sim->tick_counter; r.noise_std = sim->noise_std; r.noise_seed = sim->noise_seed;
     r.lidar = scan_slots; r.final_slots = final_slots;
-    const TtcK q = fill_ttc_k(sim, map, beams, tp, ep->list, ep->list_count);
-    if (units == F110_SCAN_UNITS_ROT) launch_restart_march_t<F110_SCAN_UNITS_ROT>(q, r, tp.march.count, grid, st);
-    else if (units == F110_SCAN_UNITS_CELLS) launch_restart_march_t<F110_SCAN_UNITS_CELLS>(q, r, tp.march.count, grid, st);
-    else launch_restart_march_t<F110_SCAN_UNITS_METRES>(q, r, tp.march.count, grid, st);
-    LAUNCH_CHECK("k_restart_march");
-    const BeamView bv = make_view(beams);
-    const double max_scan = max_scan_range(sim, map);
-    const unsigned slots = (unsigned)__builtin_popcount(scan_slots);
-    if (A > 1 && slots) {
-        const LidarOrder lo = {scan_slots, slots};
-        k_episode_cast<<<(unsigned)(((unsigned long long)N * slots + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS),
-                         32 * F110_LIDAR_CAST_WARPS, 0, st>>>(*sim, bv, lo, ep->list, ep->list_count, max_scan);
-        LAUNCH_CHECK("k_episode_cast");
-    }
-    k_episode_tail<<<(N + 127) / 128, 128, 0, st>>>(*sim, ep->list, ep->list_count);
-    LAUNCH_CHECK("k_episode_tail");
+    return launch_restart("k_episode_end", *sim, sim->march_rec, map, beams, tp, r, grid, st);
+}
+
+// ---- a held-action call (f110_tick_repeat_ticks_lidar, f110_tick_repeat_episodes_ticks): its checks, before anything is planned
+static int check_repeat(const f110_sim *sim, const f110_map *map, int32_t repeat, int32_t first_tick, int32_t num_ticks,
+                        const f110_repeat *rep, int32_t env_level, const double *start_poses, int32_t num_start, int32_t pose_gap,
+                        uint64_t seed, const f110_lidar *lidar, TailOpts *t) {
+    int rc;
+    if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, t))) return rc;
+    if ((rc = check_lidar(sim, lidar))) return rc;
+    if (repeat < 1 || repeat > F110_MAX_REPEAT || first_tick < 0 || num_ticks < 1 || first_tick > repeat - num_ticks) return F110_ERR_INVALID;
+    if (!rep || !rep->list || !rep->list_count) return F110_ERR_INVALID;
+    if ((rep->done_any || rep->done_tick) && !env_level) return F110_ERR_INVALID;     // done is computed by the env-level part
+    return F110_OK;
+}
+// its plans: the ticks', the last tick's with a lidar mask, the obstacles'
+static int plan_repeat_call(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                            const double *actions, int32_t repeat, const f110_obstacles *obst, const f110_lidar *lidar,
+                            RepeatCall *c) {
+    int rc;
+    g_launch_rec[0] = '\0';
+    if ((rc = plan_repeat(sim, map, tables, beams, actions, repeat, &c->rp))) return rc;
+    c->masked = lidar && lidar->mask != F110_LIDAR_ALL;
+    if (c->masked && (rc = plan_tick(sim, map, tables, beams, actions, &c->last, lidar))) return rc;
     if (obst) {
-        ObstK o = ob.k;
-        o.lidar = scan_slots;
-        k_episode_obstacles<<<(unsigned)(((long long)NA * 32 + 127) / 128), 128, 0, st>>>(*sim, bv, o, max_scan, ep->list,
-                                                                                          ep->list_count);
-        LAUNCH_CHECK("k_episode_obstacles");
+        if ((rc = plan_obstacles(sim, obst, map->num_layers, &c->ob))) return rc;
+        c->rp.tick.obst = &c->ob;
+        c->last.obst = &c->ob;
     }
-    append_launch_record(" episodes restart=k_episode_end+k_episode_dyn+k_restart_march%s+k_episode_tail%s restart_grid=%u",
-                         (A > 1 && slots) ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "", grid);
+    return F110_OK;
+}
+// its ticks first_tick .. first_tick + num_ticks - 1, each followed by k_repeat_done (a plain tick, when rep has the done
+// outputs) and k_episode_latch (when latch is given; its tick and scans_exist are the last tick's on return), then the record
+static int launch_repeat_ticks(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                               const double *actions, int32_t repeat, int32_t first_tick, int32_t num_ticks, const f110_repeat *rep,
+                               RepeatCall &c, LatchK *latch, cudaStream_t st) {
+    int rc;
+    const RepeatPlan &rp = c.rp;
+    const bool track_done = rep->done_any || rep->done_tick;
+    for (int tick = first_tick; tick < first_tick + num_ticks; tick++) {
+        const bool short_tick = rp.ttc && tick < repeat - 1;
+        if (short_tick) {
+            if ((rc = launch_ttc_tick(sim, map, beams, actions, rp, rep, tick, c.t, st))) return rc;
+        } else {
+            if ((rc = launch_tick(sim, map, tables, beams, actions, tick == repeat - 1 ? c.last_tick() : c.rp.tick, st, nullptr, &c.t)))
+                return rc;
+            if (track_done) {
+                RepeatDone rd;
+                rd.done_any = rep->done_any; rd.done_tick = rep->done_tick; rd.tick = tick;
+                k_repeat_done<<<(sim->num_envs + 127) / 128, 128, 0, st>>>(*sim, rd);
+                LAUNCH_CHECK("k_repeat_done");
+            }
+        }
+        if (latch) {
+            latch->tick = tick;
+            latch->scans_exist = short_tick ? 0 : 1;
+            k_episode_latch<<<(unsigned)(((long long)sim->num_envs * 32 + 127) / 128), 128, 0, st>>>(*sim, *latch);
+            LAUNCH_CHECK("k_episode_latch");
+        }
+    }
+    // the record of the call: the last plain tick's record (when the range holds one) and the repeat part
+    static const char *units[3] = {"cells", "metres", "rot"};
+    append_launch_record("%srepeat=%d sub=%s UNITS=%s grid=%u", g_launch_rec[0] ? " " : "", (int)repeat, rp.ttc ? "ttc" : "full",
+                         units[rp.units], rp.grid);
     return F110_OK;
 }
 
@@ -2974,48 +3066,14 @@ int f110_tick_repeat_ticks_lidar(const f110_sim *sim, const f110_map *map, const
                                  int32_t num_start, int32_t pose_gap, uint64_t seed, const f110_obstacles *obst,
                                  const f110_lidar *lidar, void *stream) {
     int rc;
-    TailOpts t;
-    RepeatPlan rp;
-    TickPlan last;           // the last tick of the call: the plain tick's plan, with the lidar mask
-    ObstPlan ob;
+    RepeatCall c;
     cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = tick_tail_opts(sim, map, env_level, start_poses, num_start, pose_gap, seed, &t))) return rc;
-    if ((rc = check_lidar(sim, lidar))) return rc;
-    if (repeat < 1 || repeat > F110_MAX_REPEAT || first_tick < 0 || num_ticks < 1 || first_tick > repeat - num_ticks) return F110_ERR_INVALID;
-    if (!rep || !rep->list || !rep->list_count) return F110_ERR_INVALID;
-    if ((rep->done_any || rep->done_tick) && !env_level) return F110_ERR_INVALID;     // done is computed by the env-level part
-    g_launch_rec[0] = '\0';
-    if ((rc = plan_repeat(sim, map, tables, beams, actions, repeat, &rp))) return rc;
-    const bool masked = lidar && lidar->mask != F110_LIDAR_ALL;
-    if (masked && (rc = plan_tick(sim, map, tables, beams, actions, &last, lidar))) return rc;
-    if (obst) {
-        if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
-        rp.tick.obst = &ob;
-        last.obst = &ob;
-    }
-
+    if ((rc = check_repeat(sim, map, repeat, first_tick, num_ticks, rep, env_level, start_poses, num_start, pose_gap, seed, lidar,
+                           &c.t)))
+        return rc;
+    if ((rc = plan_repeat_call(sim, map, tables, beams, actions, repeat, obst, lidar, &c))) return rc;
     if (first_tick == 0) CUDA_TRY(cudaMemsetAsync(rep->list_count, 0, sizeof(uint32_t) * (size_t)repeat, st));
-    const bool track_done = rep->done_any || rep->done_tick;
-    for (int tick = first_tick; tick < first_tick + num_ticks; tick++) {
-        if (rp.ttc && tick < repeat - 1) {
-            if ((rc = launch_ttc_tick(sim, map, beams, actions, rp, rep, tick, t, st))) return rc;
-            continue;
-        }
-        if ((rc = launch_tick(sim, map, tables, beams, actions, (masked && tick == repeat - 1) ? last : rp.tick, st, nullptr, &t)))
-            return rc;
-        if (track_done) {
-            RepeatDone rd;
-            rd.done_any = rep->done_any; rd.done_tick = rep->done_tick; rd.tick = tick;
-            k_repeat_done<<<(sim->num_envs + 127) / 128, 128, 0, st>>>(*sim, rd);
-            LAUNCH_CHECK("k_repeat_done");
-        }
-    }
-    // the record of the call: the last plain tick's record (when the range holds one) and the repeat part
-    const size_t n = strlen(g_launch_rec);
-    static const char *units[3] = {"cells", "metres", "rot"};
-    snprintf(g_launch_rec + n, sizeof(g_launch_rec) - n, "%srepeat=%d sub=%s UNITS=%s grid=%u", n ? " " : "", (int)repeat,
-             rp.ttc ? "ttc" : "full", units[rp.units], rp.grid);
-    return F110_OK;
+    return launch_repeat_ticks(sim, map, tables, beams, actions, repeat, first_tick, num_ticks, rep, c, nullptr, st);
 }
 
 int f110_tick_repeat(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
@@ -3033,55 +3091,34 @@ int f110_tick_repeat_episodes_ticks(const f110_sim *sim, const f110_map *map, co
                                     int32_t pose_gap, uint64_t seed, const f110_obstacles *obst, const f110_lidar *lidar,
                                     const f110_episodes *ep, const f110_episode_repeat *er, void *stream) {
     int rc;
-    TailOpts t;
-    RepeatPlan rp;
-    TickPlan last;           // the last tick of the call: the plain tick's plan, with the lidar mask
-    ObstPlan ob;
+    RepeatCall c;
     cudaStream_t st = (cudaStream_t)stream;
-    if ((rc = tick_tail_opts(sim, map, 1, start_poses, num_start, pose_gap, seed, &t))) return rc;
-    if ((rc = check_lidar(sim, lidar))) return rc;
-    if (repeat < 1 || repeat > F110_MAX_REPEAT || first_tick < 0 || num_ticks < 1 || first_tick > repeat - num_ticks) return F110_ERR_INVALID;
-    if (!rep || !rep->list || !rep->list_count) return F110_ERR_INVALID;
+    if ((rc = check_repeat(sim, map, repeat, first_tick, num_ticks, rep, 1, start_poses, num_start, pose_gap, seed, lidar, &c.t)))
+        return rc;
     if ((rc = check_episodes(sim, ep, start_poses))) return rc;
     if (!er || !er->end_tick || !er->snap_rec || !er->snap_poses || !er->snap_wall_flag || !er->scan_list || !er->scan_count)
         return F110_ERR_INVALID;
-    const AutoResetArgs ar = t.ar;
-    t.ar.start_poses = nullptr;          // the ticks run without the auto-reset; k_episode_restart restarts the ended envs
-    g_launch_rec[0] = '\0';
-    if ((rc = plan_repeat(sim, map, tables, beams, actions, repeat, &rp))) return rc;
-    if (!episode_march_ok(rp.tick.march)) return F110_ERR_INVALID;
-    const bool masked = lidar && lidar->mask != F110_LIDAR_ALL;
-    if (masked && (rc = plan_tick(sim, map, tables, beams, actions, &last, lidar))) return rc;
-    if (obst) {
-        if ((rc = plan_obstacles(sim, obst, map->num_layers, &ob))) return rc;
-        rp.tick.obst = &ob;
-        last.obst = &ob;
-    }
-    TickPlan &lp = masked ? last : rp.tick;
-    if (!episode_march_ok(lp.march)) return F110_ERR_INVALID;      // the plan the last tick and the restart march run with
-    const int units = lp.march.rot ? F110_SCAN_UNITS_ROT : lp.march.cell_units ? F110_SCAN_UNITS_CELLS : F110_SCAN_UNITS_METRES;
+    const AutoResetArgs ar = c.t.ar;
+    c.t.ar.start_poses = nullptr;        // the ticks run without the auto-reset; k_episode_restart restarts the ended envs
+    if ((rc = plan_repeat_call(sim, map, tables, beams, actions, repeat, obst, lidar, &c))) return rc;
+    const RepeatPlan &rp = c.rp;
+    const TickPlan &lp = c.last_tick();
+    // the plans the final-scan pass and the last tick and the restart march run with
+    if (!episode_march_ok(rp.tick.march) || !episode_march_ok(lp.march)) return F110_ERR_INVALID;
+    const int units = scan_units(lp.march);
     unsigned grid = 0u, fs_grid = 0u;
-    if ((rc = units == F110_SCAN_UNITS_ROT ? restart_grid<F110_SCAN_UNITS_ROT>(lp.march.count, &grid)
-            : units == F110_SCAN_UNITS_CELLS ? restart_grid<F110_SCAN_UNITS_CELLS>(lp.march.count, &grid)
-                                             : restart_grid<F110_SCAN_UNITS_METRES>(lp.march.count, &grid)))
-        return rc;
-    if (rp.ttc && (rc = units == F110_SCAN_UNITS_ROT ? restart_grid<F110_SCAN_UNITS_ROT>(false, &fs_grid)
-                       : units == F110_SCAN_UNITS_CELLS ? restart_grid<F110_SCAN_UNITS_CELLS>(false, &fs_grid)
-                                                        : restart_grid<F110_SCAN_UNITS_METRES>(false, &fs_grid)))
-        return rc;
+    if ((rc = ttc_grid(true, units, lp.march.count, &grid))) return rc;
+    if (rp.ttc && (rc = ttc_grid(true, units, false, &fs_grid))) return rc;
 
-    const int N = sim->num_envs, A = sim->num_agents, NA = N * A;
+    const int N = sim->num_envs, A = sim->num_agents;
     const uint32_t all = A == 32 ? 0xFFFFFFFFu : (1u << A) - 1u;
     // the slots whose scans the last tick computes, and the slots that have a lidar (their scans go to final_scans)
     const uint32_t scan_slots = lp.lidar ? lp.lidar->mask : all;
-    const uint32_t final_slots = masked ? (lidar->mask & all) : all;
+    const uint32_t final_slots = c.masked ? (lidar->mask & all) : all;
     f110_repeat rn = *rep;               // the ticks' own done bookkeeping is off: k_episode_latch keeps it to the running episode
     rn.done_any = nullptr; rn.done_tick = nullptr;
     LatchK k;
-    k.ep.ticks = ep->ticks; k.ep.length = ep->length; k.ep.terminated = ep->terminated; k.ep.truncated = ep->truncated;
-    k.ep.final_state = ep->final_state; k.ep.final_collisions = ep->final_collisions; k.ep.final_lap_times = ep->final_lap_times;
-    k.ep.final_lap_counts = ep->final_lap_counts; k.ep.final_collision_idx = ep->final_collision_idx;
-    k.ep.list = ep->list; k.ep.count = ep->list_count; k.ep.track_seg = ep->track_seg; k.ep.max_ticks = ep->max_ticks;
+    k.ep = episode_k(ep);
     k.end_tick = er->end_tick; k.done_any = rep->done_any; k.done_tick = rep->done_tick;
     k.scans = sim->scans; k.final_scans = ep->final_scans;
     k.snap_rec = reinterpret_cast<double2 *>(er->snap_rec); k.snap_poses = er->snap_poses; k.snap_flag = er->snap_wall_flag;
@@ -3092,98 +3129,35 @@ int f110_tick_repeat_episodes_ticks(const f110_sim *sim, const f110_map *map, co
         CUDA_TRY(cudaMemsetAsync(rep->list_count, 0, sizeof(uint32_t) * (size_t)repeat, st));
         CUDA_TRY(cudaMemsetAsync(er->scan_count, 0, sizeof(uint32_t), st));
     }
-    for (int tick = first_tick; tick < first_tick + num_ticks; tick++) {
-        const bool short_tick = rp.ttc && tick < repeat - 1;
-        if (short_tick) {
-            if ((rc = launch_ttc_tick(sim, map, beams, actions, rp, &rn, tick, t, st))) return rc;
-        } else if ((rc = launch_tick(sim, map, tables, beams, actions, tick == repeat - 1 ? lp : rp.tick, st,
-                                     nullptr, &t))) {
-            return rc;
-        }
-        k.tick = tick;
-        k.scans_exist = short_tick ? 0 : 1;
-        k_episode_latch<<<(unsigned)(((long long)N * 32 + 127) / 128), 128, 0, st>>>(*sim, k);
-        LAUNCH_CHECK("k_episode_latch");
-    }
-    const size_t n = strlen(g_launch_rec);
-    static const char *unit_names[3] = {"cells", "metres", "rot"};
-    snprintf(g_launch_rec + n, sizeof(g_launch_rec) - n, "%srepeat=%d sub=%s UNITS=%s grid=%u", n ? " " : "", (int)repeat,
-             rp.ttc ? "ttc" : "full", unit_names[rp.units], rp.grid);
+    if ((rc = launch_repeat_ticks(sim, map, tables, beams, actions, repeat, first_tick, num_ticks, &rn, c, &k, st))) return rc;
     if (first_tick + num_ticks < repeat) return F110_OK;
 
-    const BeamView bv = make_view(beams);
-    const double max_scan = max_scan_range(sim, map);
-    const unsigned fslots = (unsigned)__builtin_popcount(final_slots);
     // the final scans of the envs that ended on a short-path tick, from the snapshot of their end tick
-    const bool final_pass = rp.ttc && repeat > 1 && fslots;
+    const bool final_pass = rp.ttc && repeat > 1 && final_slots != 0u;
     if (final_pass) {
         f110_sim fs = *sim;
-        fs.agent_poses = er->snap_poses; fs.wall_flag = er->snap_wall_flag; fs.scans = ep->final_scans;
+        fs.agent_poses = er->snap_poses; fs.scans = ep->final_scans;
+        fs.wall_flag = er->snap_wall_flag;          // never written: the snapshot's iTTC threshold is -inf
         fs.collisions = ep->final_collisions; fs.collision_idx = ep->final_collision_idx;
-        TtcK q = fill_ttc_k(sim, map, beams, rp.tick, er->scan_list, er->scan_count);
-        q.rec = reinterpret_cast<const double2 *>(er->snap_rec);
-        q.wall_flag = er->snap_wall_flag;           // never written: the snapshot's iTTC threshold is -inf
         RestartK r;
         r.list = er->scan_list; r.count = er->scan_count; r.scans = ep->final_scans; r.final_scans = ep->final_scans;
         r.tick_counter = sim->tick_counter; r.noise_std = 0.0; r.noise_seed = 0ull;
         r.lidar = final_slots; r.final_slots = 0u;
-        if (units == F110_SCAN_UNITS_ROT) launch_restart_march_t<F110_SCAN_UNITS_ROT>(q, r, false, fs_grid, st);
-        else if (units == F110_SCAN_UNITS_CELLS) launch_restart_march_t<F110_SCAN_UNITS_CELLS>(q, r, false, fs_grid, st);
-        else launch_restart_march_t<F110_SCAN_UNITS_METRES>(q, r, false, fs_grid, st);
-        LAUNCH_CHECK("k_restart_march");
-        if (A > 1) {
-            const LidarOrder lo = {final_slots, fslots};
-            k_episode_cast<<<(unsigned)(((unsigned long long)N * fslots + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS),
-                             32 * F110_LIDAR_CAST_WARPS, 0, st>>>(fs, bv, lo, er->scan_list, er->scan_count, max_scan);
-            LAUNCH_CHECK("k_episode_cast");
-        }
-        if (obst) {
-            ObstK o = ob.k;
-            o.lidar = final_slots;
-            o.hit = nullptr;
-            k_episode_obstacles<<<(unsigned)(((long long)NA * 32 + 127) / 128), 128, 0, st>>>(fs, bv, o, max_scan, er->scan_list,
-                                                                                              er->scan_count);
-            LAUNCH_CHECK("k_episode_obstacles");
-        }
+        if ((rc = launch_restart(nullptr, fs, er->snap_rec, map, beams, rp.tick, r, fs_grid, st))) return rc;
     }
 
     // the restart of every env that ended in the call, at the counter of its last tick
     ObstDraw no_draw;
     memset(&no_draw, 0, sizeof(no_draw));
     CUDA_TRY(cudaMemsetAsync(ep->list_count, 0, sizeof(uint32_t), st));
-    k_episode_restart<<<(N + 127) / 128, 128, 0, st>>>(*sim, ar, k, obst ? ob.d : no_draw, ep->track_seg, er->track_delta_sum,
+    k_episode_restart<<<(N + 127) / 128, 128, 0, st>>>(*sim, ar, k, obst ? c.ob.d : no_draw, ep->track_seg, er->track_delta_sum,
                                                       ep->list, ep->list_count);
     LAUNCH_CHECK("k_episode_restart");
-    k_episode_dyn<<<(NA + 127) / 128, 128, 0, st>>>(*sim, beams->fov, (double)map->theta_dis,
-                                                    fill_first_lookup(sim, map, beams, lp.geom, lp.march), ep->list, ep->list_count);
-    LAUNCH_CHECK("k_episode_dyn");
     RestartK r;
     r.list = ep->list; r.count = ep->list_count; r.scans = sim->scans; r.final_scans = ep->final_scans;
     r.tick_counter = sim->tick_counter; r.noise_std = sim->noise_std; r.noise_seed = sim->noise_seed;
     r.lidar = scan_slots; r.final_slots = 0u;    // the crash scans are in final_scans already (k_episode_latch)
-    const TtcK q = fill_ttc_k(sim, map, beams, lp, ep->list, ep->list_count);
-    if (units == F110_SCAN_UNITS_ROT) launch_restart_march_t<F110_SCAN_UNITS_ROT>(q, r, lp.march.count, grid, st);
-    else if (units == F110_SCAN_UNITS_CELLS) launch_restart_march_t<F110_SCAN_UNITS_CELLS>(q, r, lp.march.count, grid, st);
-    else launch_restart_march_t<F110_SCAN_UNITS_METRES>(q, r, lp.march.count, grid, st);
-    LAUNCH_CHECK("k_restart_march");
-    const unsigned slots = (unsigned)__builtin_popcount(scan_slots);
-    if (A > 1 && slots) {
-        const LidarOrder lo = {scan_slots, slots};
-        k_episode_cast<<<(unsigned)(((unsigned long long)N * slots + F110_LIDAR_CAST_WARPS - 1) / F110_LIDAR_CAST_WARPS),
-                         32 * F110_LIDAR_CAST_WARPS, 0, st>>>(*sim, bv, lo, ep->list, ep->list_count, max_scan);
-        LAUNCH_CHECK("k_episode_cast");
-    }
-    k_episode_tail<<<(N + 127) / 128, 128, 0, st>>>(*sim, ep->list, ep->list_count);
-    LAUNCH_CHECK("k_episode_tail");
-    if (obst) {
-        ObstK o = ob.k;
-        o.lidar = scan_slots;
-        k_episode_obstacles<<<(unsigned)(((long long)NA * 32 + 127) / 128), 128, 0, st>>>(*sim, bv, o, max_scan, ep->list,
-                                                                                          ep->list_count);
-        LAUNCH_CHECK("k_episode_obstacles");
-    }
-    append_launch_record(" episodes restart=k_episode_restart+k_episode_dyn+k_restart_march%s+k_episode_tail%s restart_grid=%u",
-                         (A > 1 && slots) ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "", grid);
+    if ((rc = launch_restart("k_episode_restart", *sim, sim->march_rec, map, beams, lp, r, grid, st))) return rc;
     if (final_pass)
         append_launch_record(" final_scan=k_restart_march%s%s", A > 1 ? "+k_episode_cast" : "", obst ? "+k_episode_obstacles" : "");
     else
@@ -3239,6 +3213,13 @@ int f110_params_draw_episodes(const f110_sim *sim, const f110_param_draw *draw, 
     return param_draw_launch(sim, draw, PARAM_DRAW_EPISODES, nullptr, ep, stream);
 }
 
+// the tail of a host-buffer step: the fused tail, with the env level when the sim has its arrays, and no auto-reset
+static TailOpts host_step_tail(bool env_level) {
+    TailOpts t;
+    t.fused = true; t.env_level = env_level ? 1 : 0;
+    t.ar.start_poses = nullptr; t.ar.num_start = 0; t.ar.pose_gap = 0; t.ar.seed = 0; t.ar.tick_host = 0;
+    return t;
+}
 int f110_step_host(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const double *actions_host,
                    double *actions_dev_scratch, const f110_host_obs *out, void *stream) {
     int rc;
@@ -3249,9 +3230,7 @@ int f110_step_host(const f110_sim *sim, const f110_map *map, const f110_beams *b
     CUDA_TRY(cudaMemcpyAsync(actions_dev_scratch, actions_host, NA * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
     const bool env_level = sim->current_time && sim->done;
     if (env_level && (rc = check_env_arrays(sim))) return rc;
-    TailOpts t;
-    t.fused = true; t.env_level = env_level ? 1 : 0;
-    t.ar.start_poses = nullptr; t.ar.num_start = 0; t.ar.pose_gap = 0; t.ar.seed = 0; t.ar.tick_host = 0;
+    const TailOpts t = host_step_tail(env_level);
     if ((rc = step_impl(sim, map, nullptr, beams, actions_dev_scratch, st, nullptr, &t))) return rc;
     if (out->scans)
         CUDA_TRY(cudaMemcpyAsync(out->scans, sim->scans, NA * beams->num_beams * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -3291,9 +3270,7 @@ int f110_step_host_async_ex(const f110_sim *sim, const f110_map *map, const f110
     const bool env_level = sim->current_time && sim->done;
     if (env_level && (rc = check_env_arrays(sim))) return rc;
     CUDA_TRY(cudaMemcpyAsync(actions_dev_scratch, actions_host, NA * 2 * sizeof(double), cudaMemcpyHostToDevice, cs));
-    TailOpts t;
-    t.fused = true; t.env_level = env_level ? 1 : 0;
-    t.ar.start_poses = nullptr; t.ar.num_start = 0; t.ar.pose_gap = 0; t.ar.seed = 0; t.ar.tick_host = 0;
+    const TailOpts t = host_step_tail(env_level);
     if ((rc = step_impl(sim, map, tables, beams, actions_dev_scratch, cs, nullptr, &t))) return rc;
     // the staging buffers may still be draining to the host from their previous use
     CUDA_TRY(cudaStreamWaitEvent(cs, e_copy, 0));

@@ -671,18 +671,32 @@ class Simulator(object):
         a = self._actions_tensor(control_inputs)
         table, n = self._start_table(autoreset_poses)
         L = nat.lib()
-        if self._episode_path(table, env_level):
-            self._launch_episodes(L, a, table, n, pose_gap, seed)
-            self._draw_episodes(L)
-            obs = self.observations()
+        episodes = self._episode_path(table, env_level)
+        self._enqueue_tick(L, a, env_level, table, n, pose_gap, seed, episodes, progress=False)
+        obs = self.observations()
+        if episodes:
             obs['terminated'], obs['truncated'] = self.ep_terminated, self.ep_truncated
-            return obs
-        nat.check(L.f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                    C.byref(self.beams.c), nat.ptr(a), 1 if env_level else 0, nat.ptr(table), n, pose_gap,
-                                    int(seed), self._obst_ref(), self._lidar_ref(), _stream_ptr(self.device)))
-        if table is not None:
-            self._draw_autoreset(L)
-        return self.observations()
+        return obs
+
+    def _enqueue_tick(self, L, actions, env_level, table, num_start, pose_gap, seed, episodes, progress):
+        """Enqueue one tick: the episode tick (f110_tick_episodes) or f110_tick_lidar, the parameter draw of the envs it
+        restarted, then update_progress() with progress."""
+        if episodes:
+            self._episodes.track_seg = nat.ptr(self.track_seg)
+            nat.check(L.f110_tick_episodes(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                           C.byref(self.beams.c), nat.ptr(actions), nat.ptr(table), num_start, pose_gap,
+                                           int(seed), self._obst_ref(), self._lidar_ref(), C.byref(self._episodes),
+                                           _stream_ptr(self.device)))
+            self._draw_episodes(L)
+        else:
+            nat.check(L.f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
+                                        C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table),
+                                        num_start, pose_gap, int(seed), self._obst_ref(), self._lidar_ref(),
+                                        _stream_ptr(self.device)))
+            if table is not None:
+                self._draw_autoreset(L)
+        if progress:
+            self._launch_progress(L)
 
     # ------------------------------------------------------------------ episodes
     def set_episodes(self, max_ticks=None):
@@ -789,12 +803,6 @@ class Simulator(object):
     def _no_episodes(self, who):
         if self._episodes is not None:
             raise ValueError('%s does not run episode mode; call set_episodes(False) first or use tick / capture_graph' % who)
-
-    def _launch_episodes(self, L, actions, table, num_start, pose_gap, seed):
-        self._episodes.track_seg = nat.ptr(self.track_seg)
-        nat.check(L.f110_tick_episodes(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                       C.byref(self.beams.c), nat.ptr(actions), nat.ptr(table), num_start, pose_gap, int(seed),
-                                       self._obst_ref(), self._lidar_ref(), C.byref(self._episodes), _stream_ptr(self.device)))
 
     # ------------------------------------------------------------------ agents without a lidar
     def set_lidar(self, slots):
@@ -1243,21 +1251,8 @@ class Simulator(object):
         def tick():
             if K > 1:
                 self._issue_repeat(L, actions, K, call, env_level, table, num_start, pose_gap, autoreset_seed, progress, episodes)
-                return
-            if episodes:
-                self._launch_episodes(L, actions, table, num_start, pose_gap, autoreset_seed)
-                self._draw_episodes(L)
-                if progress:
-                    self._launch_progress(L)
-                return
-            nat.check(L.f110_tick_lidar(C.byref(self.c), C.byref(self._map_struct), C.byref(self._march_tables),
-                                        C.byref(self.beams.c), nat.ptr(actions), 1 if env_level else 0, nat.ptr(table), num_start,
-                                        pose_gap, int(autoreset_seed), self._obst_ref(), self._lidar_ref(),
-                                        _stream_ptr(self.device)))
-            if table is not None:
-                self._draw_autoreset(L)
-            if progress:
-                self._launch_progress(L)
+            else:
+                self._enqueue_tick(L, actions, env_level, table, num_start, pose_gap, autoreset_seed, episodes, progress)
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
