@@ -118,6 +118,14 @@ class F110ParamDraw(C.Structure):
                 ('seed', C.c_uint64), ('final_params', _dp)]
 
 
+class F110PredictArgs(C.Structure):
+    """include/f110_predict.h f110_predict_args."""
+    _fields_ = [('agent_ids', _dp), ('actions', _dp), ('M', C.c_int32), ('K', C.c_int32), ('H', C.c_int32), ('final_state', _dp),
+                ('wall_step', _dp), ('states', _dp), ('clearance', _dp)]
+
+
+PREDICT_MAX_H = 4096
+
 PARAM_DRAW_KEYS = 16     # keys 0..15 are drawable; width and length are not
 PARAM_DRAW_C = (0xC2B2AE3D27D4EB4F, 0x165667B19E3779F9, 0x27D4EB2F165667C5, 0x85EBCA77C2B2AE63)   # C1..C4 (tick, env, slot, group)
 
@@ -218,6 +226,11 @@ PARAM_DRAW_SIGNATURES = {
     'f110_params_draw_episodes': (C.c_int, [_P(F110Sim), _P(F110ParamDraw), _P(F110Episodes), _dp]),
 }
 
+# the entry point of include/f110_predict.h (predicted futures), bound like SIGNATURES
+PREDICT_SIGNATURES = {
+    'f110_predict': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _P(F110PredictArgs), _dp]),
+}
+
 DEBUG_SIGNATURES = {
     'f110_debug_set_variant': (None, [C.c_int]),
     'f110_debug_set_chunk': (None, [C.c_int]),
@@ -258,7 +271,7 @@ def lib():
     except OSError as e:
         raise NativeLibraryError('f1tenth_gym_b200: cannot load %s: %s' % (LIB_PATH, e))
     for name, (res, args) in list(SIGNATURES.items()) + list(EPISODE_SIGNATURES.items()) + list(EPISODE_REPEAT_SIGNATURES.items()) + \
-            list(PARAM_DRAW_SIGNATURES.items()):
+            list(PARAM_DRAW_SIGNATURES.items()) + list(PREDICT_SIGNATURES.items()):
         try:
             f = getattr(L, name)
         except AttributeError:

@@ -31,6 +31,7 @@
 #include "../../include/f110_episodes.h"
 #include "../../include/f110_episode_repeat.h"
 #include "../../include/f110_param_draw.h"
+#include "../../include/f110_predict.h"
 #include "collision.cuh"
 #include "dynamics.cuh"
 #include "lidar.cuh"
@@ -1221,6 +1222,7 @@ __global__ void __launch_bounds__(32 * F110_LIDAR_CAST_WARPS) k_lidar_cast(f110_
 #include "episodes.cuh"      // the restart of ended episodes: built on the same functions and on obstacles.cuh's
 #include "episode_repeat.cuh"   // episodes under a held action: the end latch, reusing the restart kernels above
 #include "param_draw.cuh"       // per-episode parameter draws, launched after the call that restarted the envs
+#include "predict.cuh"          // predicted futures: k_dynamics' and k_march_ttc's per-agent statements in one rollout kernel
 namespace f110 {
 
 // f110_track_progress_sum: the deltas of the ticks of one policy step, summed in tick order
@@ -2317,11 +2319,15 @@ static int launch_obst_tail(const f110_sim *sim, const BeamView &bv, const ObstP
 // needs: no scan noise (the bound does not hold for a Gaussian, and the Philox stream must stay the plain run's); a lean march
 // family, which brings the per-agent record, the doubled LUT and `dt_min_positive > eps`; a known max side distance below
 // max_range (otherwise every moving agent is listed); and at most 32 agents per env (the block-owns-envs tail).
-static bool ttc_path_ok(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const MarchPlan &m) {
+// The map and beam part of those conditions is also what f110_predict needs: the per-agent record's arithmetic and k_march_ttc's.
+static bool ttc_tables_ok(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const MarchPlan &m) {
     const bool lean_family = m.family == MarchFamily::LEAN || m.family == MarchFamily::LEAN_BRICK || m.family == MarchFamily::LEAN_HET ||
                              m.family == MarchFamily::LEAN_HET_RES || m.family == MarchFamily::LEAN_ROT;
-    return sim->noise_std == 0.0 && m.lean && lean_family && sim->march_rec && map->sincos2 && map->dt_min_positive > map->eps &&
-           beams->side_max > 0.0 && beams->side_max < map->max_range && sim->num_agents <= 32;
+    return m.lean && lean_family && sim->march_rec && map->sincos2 && map->dt_min_positive > map->eps && beams->side_max > 0.0 &&
+           beams->side_max < map->max_range;
+}
+static bool ttc_path_ok(const f110_sim *sim, const f110_map *map, const f110_beams *beams, const MarchPlan &m) {
+    return sim->noise_std == 0.0 && ttc_tables_ok(sim, map, beams, m) && sim->num_agents <= 32;
 }
 // The units (F110_SCAN_UNITS_*) k_march_ttc and k_restart_march run in for a march plan.  They follow the family, never the
 // queue length, so a tick's plan and its lidar-mask plan agree.
@@ -3203,6 +3209,42 @@ static int param_draw_launch(const f110_sim *sim, const f110_param_draw *draw, i
     LAUNCH_CHECK("k_param_draw");
     return F110_OK;
 }
+// ---- f110_predict (include/f110_predict.h, csrc/predict.cuh)
+// The tick's own plan decides the map kind: the record arithmetic (fill_first_lookup) and the per-beam march (fill_ttc_k) of
+// k_march_ttc on it, with the units of the tick's short path.  Validation ends before the one launch.
+int f110_predict(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                 const f110_predict_args *args, void *stream) {
+    int rc;
+    if (!sim || !args || !args->agent_ids || !args->actions || !args->final_state || !args->wall_step) return F110_ERR_INVALID;
+    if (args->M < 1 || args->K < 1 || args->H < 1 || args->H > F110_PREDICT_MAX_H) return F110_ERR_INVALID;
+    const long long samples = (long long)args->M * (long long)args->K;
+    if (samples > 0x7fffffffll) return F110_ERR_INVALID;
+    if ((rc = check_sim(sim)) || (rc = check_map(map)) || (rc = check_beams(beams))) return rc;
+    if ((long long)sim->num_envs * sim->num_agents > 0x7fffffffll) return F110_ERR_INVALID;
+    TickPlan tp = {};
+    if ((rc = classify_map(map, &tp.geom))) return rc;
+    if ((rc = plan_march(sim, map, tables, beams, tp.geom, rm_variant(), &tp.march))) return rc;
+    if (!ttc_tables_ok(sim, map, beams, tp.march)) return F110_ERR_INVALID;
+    const MarchPlan &m = tp.march;
+    PredictK p;
+    p.agent_ids = args->agent_ids;
+    p.actions = reinterpret_cast<const double2 *>(args->actions);
+    p.final_state = args->final_state; p.wall_step = args->wall_step;
+    p.states = args->states; p.clearance = args->clearance;
+    p.samples = (unsigned long long)samples; p.K = (unsigned)args->K; p.H = args->H;
+    p.d0_scale = m.cell_units ? map->resolution : 1.0;
+    p.fov = beams->fov; p.theta_dis_f = (double)map->theta_dis;
+    const FirstLookup fl = fill_first_lookup(sim, map, beams, tp.geom, m);
+    const TtcK q = fill_ttc_k(sim, map, beams, tp, nullptr, nullptr);
+    const unsigned grid = (unsigned)((samples + F110_PREDICT_THREADS - 1) / F110_PREDICT_THREADS);
+    const cudaStream_t st = (cudaStream_t)stream;
+    dispatch_units(scan_units(m), [&](auto u) {
+        k_predict<decltype(u)::value><<<grid, F110_PREDICT_THREADS, 0, st>>>(*sim, fl, q, p);
+    });
+    LAUNCH_CHECK("k_predict");
+    return F110_OK;
+}
+
 int f110_params_draw(const f110_sim *sim, const f110_param_draw *draw, const uint8_t *env_mask, void *stream) {
     return param_draw_launch(sim, draw, PARAM_DRAW_MASK, env_mask, nullptr, stream);
 }

@@ -1148,6 +1148,94 @@ class Simulator(object):
                                                _stream_ptr(self.device)))
         return out
 
+    # ------------------------------------------------------------------ predicted futures
+    def predict(self, actions, agent_ids=None, record_states=False, record_clearance=False):
+        """K candidate futures of M agents, H ticks each, in one launch (C ABI f110_predict, include/f110_predict.h), for
+        sampling-based control (MPPI, CEM, random shooting).  actions: (M, K, H, 2) fp64 (steer, speed) per step; agent_ids:
+        the M flat source agents e*A + slot (repeats allowed), None = every agent (M = N*A).  Sample (m, k) starts from agent
+        agent_ids[m]'s current state, steer FIFO, parameter row and map layer and runs, per step, that agent's tick alone: FIFO,
+        pid, RK4 / Euler, yaw wrap, scan pose, the iTTC wall check on the wall-only scan (a hit zeroes state[3:]) -- no scan
+        noise, opponents, boxes, laps, done or auto-reset.  With the scan noise off, step h equals the agent's state after h + 1
+        ticks of step / tick under the same actions, bit for bit.  Returns {'final_state': (M, K, 7), 'wall_step': (M, K) int32
+        (first step whose wall check fired, -1 for none)} plus 'states' (M, K, H, 7) with record_states and 'clearance'
+        (M, K, H) fp32 (the distance transform at each step's scan pose, metres) with record_clearance; state order x, y,
+        steer, v, yaw, yaw_rate, slip.  The tensors are views of buffers kept while (M, K, H, flags) stay the same and
+        overwritten by the next call, so a call after a first one of the same shape can be captured in a CUDA graph.
+        Ids given on the host are range-checked (ValueError); a CUDA int32 tensor goes to the kernel unchecked, and an id
+        outside [0, N*A) there gives NaN states, wall_step -1 and NaN clearance.  ValueError before any device work for a
+        bad shape, dtype, device or size, and for a map on which the held-action short path cannot run (no lean ray march,
+        side distances unknown or not below max_range)."""
+        NA = self.num_envs * self.num_agents
+        if self.map is None:
+            raise ValueError('predict needs a map: call set_map or set_device_map first')
+        mc, bc = self._map_struct, self.beams.c
+        if not (self.march_rec is not None and mc.sincos2 and mc.dt_min_positive > mc.eps and 0.0 < bc.side_max < mc.max_range):
+            raise ValueError('predict needs the lean ray march (march queue, doubled LUT, dt_min_positive > eps) and side '
+                             'distances below max_range')
+        on_dev = torch.is_tensor(actions) and actions.is_cuda
+        if on_dev:
+            if actions.dtype != torch.float64 or actions.device != self.state.device:
+                raise ValueError('actions on the device must be float64 on %s, got %s on %s'
+                                 % (self.state.device, actions.dtype, actions.device))
+            act = actions.contiguous()
+        else:
+            act = torch.as_tensor(np.asarray(actions) if not torch.is_tensor(actions) else actions, dtype=torch.float64)
+        if act.dim() != 4 or act.shape[3] != 2:
+            raise ValueError('actions must have shape (M, K, H, 2), got %s' % (tuple(act.shape),))
+        M, K, H = (int(v) for v in act.shape[:3])
+        if agent_ids is None:
+            ids = self._view_ids(None)
+        elif torch.is_tensor(agent_ids) and agent_ids.is_cuda:
+            if agent_ids.dtype != torch.int32 or agent_ids.device != self.state.device:
+                raise ValueError('agent_ids on the device must be int32 on %s' % self.state.device)
+            ids = agent_ids.reshape(-1).contiguous()
+        else:
+            ids = None
+            a = agent_ids.numpy() if torch.is_tensor(agent_ids) else np.asarray(agent_ids)
+            if a.dtype.kind not in 'iu':
+                raise ValueError('agent_ids must be integers')
+            a = a.reshape(-1)
+            if a.size and (int(a.min()) < 0 or int(a.max()) >= NA):
+                raise ValueError('agent_ids must lie in [0, %d), got [%d, %d]' % (NA, int(a.min()), int(a.max())))
+        n_ids = ids.numel() if ids is not None else a.size
+        if n_ids != M:
+            raise ValueError('actions hold %d agents, agent_ids %d' % (M, n_ids))
+        if M < 1 or K < 1 or not 1 <= H <= nat.PREDICT_MAX_H or M * K > 0x7fffffff:
+            raise ValueError('predict needs M >= 1, K >= 1, 1 <= H <= %d and M * K < 2^31, got M=%d K=%d H=%d'
+                             % (nat.PREDICT_MAX_H, M, K, H))
+        key = (M, K, H, bool(record_states), bool(record_clearance))
+        buf = getattr(self, '_predict_buf', None)
+        if buf is None or buf['key'] != key:
+            dev = self.device
+            buf = {'key': key,
+                   'final_state': torch.empty((M, K, 7), dtype=torch.float64, device=dev),
+                   'wall_step': torch.empty((M, K), dtype=torch.int32, device=dev),
+                   'states': torch.empty((M, K, H, 7), dtype=torch.float64, device=dev) if record_states else None,
+                   'clearance': torch.empty((M, K, H), dtype=torch.float32, device=dev) if record_clearance else None,
+                   'ids': torch.empty((M,), dtype=torch.int32, device=dev), 'actions': None}
+            self._predict_buf = buf
+        if ids is None:
+            buf['ids'].copy_(torch.from_numpy(a.astype(np.int32)), non_blocking=True)
+            ids = buf['ids']
+        if not on_dev:
+            if buf['actions'] is None:
+                buf['actions'] = torch.empty((M, K, H, 2), dtype=torch.float64, device=self.device)
+            buf['actions'].copy_(act, non_blocking=True)
+            act = buf['actions']
+        args = nat.F110PredictArgs(nat.ptr(ids), nat.ptr(act), M, K, H, nat.ptr(buf['final_state']), nat.ptr(buf['wall_step']),
+                                   nat.ptr(buf['states']), nat.ptr(buf['clearance']))
+        rc = nat.lib().f110_predict(C.byref(self.c), C.byref(mc), C.byref(self._march_tables), C.byref(bc), C.byref(args),
+                                    _stream_ptr(self.device))
+        if rc == -1:        # F110_ERR_INVALID: nothing was enqueued
+            raise ValueError('f110_predict refused this simulator, map or beam setup (see include/f110_predict.h)')
+        nat.check(rc)
+        out = {'final_state': buf['final_state'], 'wall_step': buf['wall_step']}
+        if record_states:
+            out['states'] = buf['states']
+        if record_clearance:
+            out['clearance'] = buf['clearance']
+        return out
+
     # ------------------------------------------------------------------ views
     def render_views(self, agent_ids=None, size=(64, 64), metres_per_pixel=0.1, forward_offset=0.0, heading_up=True,
                      out=None):
