@@ -11,6 +11,7 @@ from . import kernels, maps, trackgen                                 # noqa: F4
 from .obstacles import obstacle_candidates                            # noqa: F401
 from .kernels import ScanSimulator2D                                  # noqa: F401
 from .planner import PurePursuitPlanner                               # noqa: F401
+from .mppi import MPPIPlanner                                         # noqa: F401
 
-__all__ = ['F110Env', 'Simulator', 'Integrator', 'ScanSimulator2D', 'PurePursuitPlanner', 'DeviceMap', 'DeviceBeams', 'kernels', 'maps',
+__all__ = ['F110Env', 'Simulator', 'Integrator', 'ScanSimulator2D', 'PurePursuitPlanner', 'MPPIPlanner', 'DeviceMap', 'DeviceBeams', 'kernels', 'maps',
            'trackgen']

@@ -126,6 +126,27 @@ class F110PredictArgs(C.Structure):
 
 PREDICT_MAX_H = 4096
 
+
+class F110Cost(C.Structure):
+    """include/f110_mppi.h f110_cost."""
+    _fields_ = [('w_lat', C.c_double), ('w_head', C.c_double), ('w_clear', C.c_double), ('w_dsteer', C.c_double),
+                ('w_dspeed', C.c_double), ('w_prog', C.c_double), ('w_wall', C.c_double), ('clear_min', C.c_double),
+                ('back', C.c_int32), ('fwd', C.c_int32), ('reacquire_dist', C.c_double), ('prev_action', _dp), ('cost', _dp),
+                ('seg0', _dp), ('s0', _dp)]
+
+
+class F110Mppi(C.Structure):
+    """include/f110_mppi.h f110_mppi."""
+    _fields_ = [('M', C.c_int32), ('K', C.c_int32), ('H', C.c_int32), ('agent_ids', _dp), ('nominal', _dp), ('iteration', _dp),
+                ('no_finite', _dp), ('sigma_steer', C.c_double), ('sigma_speed', C.c_double), ('steer_lo', C.c_double),
+                ('steer_hi', C.c_double), ('speed_lo', C.c_double), ('speed_hi', C.c_double), ('lambda_', C.c_double),
+                ('seed', C.c_uint64)]
+
+
+MPPI_MAX_K = 4096
+MPPI_MAX_H = 1000
+COST_WEIGHTS = ('w_lat', 'w_head', 'w_clear', 'w_dsteer', 'w_dspeed', 'w_prog', 'w_wall')
+
 PARAM_DRAW_KEYS = 16     # keys 0..15 are drawable; width and length are not
 PARAM_DRAW_C = (0xC2B2AE3D27D4EB4F, 0x165667B19E3779F9, 0x27D4EB2F165667C5, 0x85EBCA77C2B2AE63)   # C1..C4 (tick, env, slot, group)
 
@@ -231,6 +252,14 @@ PREDICT_SIGNATURES = {
     'f110_predict': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _P(F110PredictArgs), _dp]),
 }
 
+# the entry points of include/f110_mppi.h (scored rollouts and the MPPI planner), bound like SIGNATURES
+MPPI_SIGNATURES = {
+    'f110_predict_scored': (C.c_int, [_P(F110Sim), _P(F110Map), _P(F110MarchTables), _P(F110Beams), _P(F110Track),
+                                      _P(F110PredictArgs), _P(F110Cost), _dp]),
+    'f110_mppi_sample': (C.c_int, [_P(F110Sim), _P(F110Mppi), _P(F110Episodes), _dp, _dp]),
+    'f110_mppi_update': (C.c_int, [_P(F110Mppi), _dp, _dp, _dp, C.c_int32, _dp, _dp, _dp]),
+}
+
 DEBUG_SIGNATURES = {
     'f110_debug_set_variant': (None, [C.c_int]),
     'f110_debug_set_chunk': (None, [C.c_int]),
@@ -271,7 +300,7 @@ def lib():
     except OSError as e:
         raise NativeLibraryError('f1tenth_gym_b200: cannot load %s: %s' % (LIB_PATH, e))
     for name, (res, args) in list(SIGNATURES.items()) + list(EPISODE_SIGNATURES.items()) + list(EPISODE_REPEAT_SIGNATURES.items()) + \
-            list(PARAM_DRAW_SIGNATURES.items()) + list(PREDICT_SIGNATURES.items()):
+            list(PARAM_DRAW_SIGNATURES.items()) + list(PREDICT_SIGNATURES.items()) + list(MPPI_SIGNATURES.items()):
         try:
             f = getattr(L, name)
         except AttributeError:

@@ -32,6 +32,7 @@
 #include "../../include/f110_episode_repeat.h"
 #include "../../include/f110_param_draw.h"
 #include "../../include/f110_predict.h"
+#include "../../include/f110_mppi.h"
 #include "collision.cuh"
 #include "dynamics.cuh"
 #include "lidar.cuh"
@@ -1223,6 +1224,7 @@ __global__ void __launch_bounds__(32 * F110_LIDAR_CAST_WARPS) k_lidar_cast(f110_
 #include "episode_repeat.cuh"   // episodes under a held action: the end latch, reusing the restart kernels above
 #include "param_draw.cuh"       // per-episode parameter draws, launched after the call that restarted the envs
 #include "predict.cuh"          // predicted futures: k_dynamics' and k_march_ttc's per-agent statements in one rollout kernel
+#include "mppi.cuh"             // the MPPI planner's sample and update steps around the scored rollout
 namespace f110 {
 
 // f110_track_progress_sum: the deltas of the ticks of one policy step, summed in tick order
@@ -3212,8 +3214,15 @@ static int param_draw_launch(const f110_sim *sim, const f110_param_draw *draw, i
 // ---- f110_predict (include/f110_predict.h, csrc/predict.cuh)
 // The tick's own plan decides the map kind: the record arithmetic (fill_first_lookup) and the per-beam march (fill_ttc_k) of
 // k_march_ttc on it, with the units of the tick's short path.  Validation ends before the one launch.
-int f110_predict(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
-                 const f110_predict_args *args, void *stream) {
+struct PredictCall {
+    PredictK p;
+    FirstLookup fl;
+    TtcK q;
+    int units;
+    unsigned grid;
+};
+static int plan_predict(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                        const f110_predict_args *args, PredictCall *pc) {
     int rc;
     if (!sim || !args || !args->agent_ids || !args->actions || !args->final_state || !args->wall_step) return F110_ERR_INVALID;
     if (args->M < 1 || args->K < 1 || args->H < 1 || args->H > F110_PREDICT_MAX_H) return F110_ERR_INVALID;
@@ -3226,7 +3235,7 @@ int f110_predict(const f110_sim *sim, const f110_map *map, const f110_march_tabl
     if ((rc = plan_march(sim, map, tables, beams, tp.geom, rm_variant(), &tp.march))) return rc;
     if (!ttc_tables_ok(sim, map, beams, tp.march)) return F110_ERR_INVALID;
     const MarchPlan &m = tp.march;
-    PredictK p;
+    PredictK &p = pc->p;
     p.agent_ids = args->agent_ids;
     p.actions = reinterpret_cast<const double2 *>(args->actions);
     p.final_state = args->final_state; p.wall_step = args->wall_step;
@@ -3234,14 +3243,102 @@ int f110_predict(const f110_sim *sim, const f110_map *map, const f110_march_tabl
     p.samples = (unsigned long long)samples; p.K = (unsigned)args->K; p.H = args->H;
     p.d0_scale = m.cell_units ? map->resolution : 1.0;
     p.fov = beams->fov; p.theta_dis_f = (double)map->theta_dis;
-    const FirstLookup fl = fill_first_lookup(sim, map, beams, tp.geom, m);
-    const TtcK q = fill_ttc_k(sim, map, beams, tp, nullptr, nullptr);
-    const unsigned grid = (unsigned)((samples + F110_PREDICT_THREADS - 1) / F110_PREDICT_THREADS);
+    pc->fl = fill_first_lookup(sim, map, beams, tp.geom, m);
+    pc->q = fill_ttc_k(sim, map, beams, tp, nullptr, nullptr);
+    pc->units = scan_units(m);
+    pc->grid = (unsigned)((samples + F110_PREDICT_THREADS - 1) / F110_PREDICT_THREADS);
+    return F110_OK;
+}
+int f110_predict(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                 const f110_predict_args *args, void *stream) {
+    int rc;
+    PredictCall c;
+    if ((rc = plan_predict(sim, map, tables, beams, args, &c))) return rc;
     const cudaStream_t st = (cudaStream_t)stream;
-    dispatch_units(scan_units(m), [&](auto u) {
-        k_predict<decltype(u)::value><<<grid, F110_PREDICT_THREADS, 0, st>>>(*sim, fl, q, p);
+    dispatch_units(c.units, [&](auto u) {
+        k_predict<decltype(u)::value><<<c.grid, F110_PREDICT_THREADS, 0, st>>>(*sim, c.fl, c.q, c.p);
     });
     LAUNCH_CHECK("k_predict");
+    return F110_OK;
+}
+
+// ---- f110_predict_scored (include/f110_mppi.h, csrc/predict.cuh): k_scored_acquire, then k_scored_rollout
+static bool track_ok(const f110_track *track);
+int f110_predict_scored(const f110_sim *sim, const f110_map *map, const f110_march_tables *tables, const f110_beams *beams,
+                        const f110_track *track, const f110_predict_args *args, const f110_cost *cost, void *stream) {
+    int rc;
+    if (!map || !track_ok(track) || !cost || !cost->cost || !cost->seg0 || !cost->s0) return F110_ERR_INVALID;
+    if (track->num_tables != (map->num_layers > 1 ? map->num_layers : 1)) return F110_ERR_INVALID;
+    if (cost->back < 0 || cost->fwd < 0 || (long long)cost->back + cost->fwd + 1 > F110_TRACK_MAX_WINDOW) return F110_ERR_INVALID;
+    if (!isfinite(cost->reacquire_dist) || !(cost->reacquire_dist > 0.0)) return F110_ERR_INVALID;
+    const double w[7] = {cost->w_lat, cost->w_head, cost->w_clear, cost->w_dsteer, cost->w_dspeed, cost->w_prog, cost->w_wall};
+    for (double v : w)
+        if (!isfinite(v) || !(v >= 0.0)) return F110_ERR_INVALID;
+    if (!isfinite(cost->clear_min)) return F110_ERR_INVALID;
+    PredictCall pc;
+    if ((rc = plan_predict(sim, map, tables, beams, args, &pc))) return rc;
+    CostK c;
+    c.segments = track->segments; c.table_start = track->table_start; c.num_tables = track->num_tables;
+    c.back = cost->back; c.window = cost->back + cost->fwd + 1; c.reacquire_dist = cost->reacquire_dist;
+    c.seg0 = cost->seg0; c.s0 = cost->s0;
+    c.prev_action = reinterpret_cast<const double2 *>(cost->prev_action);
+    c.cost = cost->cost;
+    c.w_lat = cost->w_lat; c.w_head = cost->w_head; c.w_clear = cost->w_clear; c.w_dsteer = cost->w_dsteer;
+    c.w_dspeed = cost->w_dspeed; c.w_prog = cost->w_prog; c.w_wall = cost->w_wall; c.clear_min = cost->clear_min;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const int M = args->M;
+    k_scored_acquire<<<(unsigned)(((long long)M * 32 + 127) / 128), 128, 0, st>>>(*sim, args->agent_ids, M, c);
+    LAUNCH_CHECK("k_scored_acquire");
+    dispatch_units(pc.units, [&](auto u) {
+        k_scored_rollout<decltype(u)::value><<<pc.grid, F110_PREDICT_THREADS, 0, st>>>(*sim, pc.fl, pc.q, pc.p, c);
+    });
+    LAUNCH_CHECK("k_scored_rollout");
+    return F110_OK;
+}
+
+// ---- f110_mppi_sample / f110_mppi_update (include/f110_mppi.h, csrc/mppi.cuh)
+static bool mppi_ok(const f110_mppi *g, MppiK *k) {
+    if (!g || !g->agent_ids || !g->nominal || !g->iteration || !g->no_finite) return false;
+    if (g->M < 1 || g->K < 2 || g->K > F110_MPPI_MAX_K || g->H < 1 || g->H > F110_MPPI_MAX_H) return false;
+    if ((long long)g->M * g->K * g->H > 0x7fffffffll) return false;
+    const double v[8] = {g->sigma_steer, g->sigma_speed, g->steer_lo, g->steer_hi, g->speed_lo, g->speed_hi, g->lambda, 0.0};
+    for (double x : v)
+        if (!isfinite(x)) return false;
+    if (!(g->sigma_steer >= 0.0) || !(g->sigma_speed >= 0.0) || !(g->lambda > 0.0)) return false;
+    if (!(g->steer_lo <= g->steer_hi) || !(g->speed_lo <= g->speed_hi)) return false;
+    k->agent_ids = g->agent_ids;
+    k->nominal = reinterpret_cast<double2 *>(g->nominal);
+    k->iteration = g->iteration; k->no_finite = g->no_finite;
+    k->sigma = make_double2(g->sigma_steer, g->sigma_speed);
+    k->lo = make_double2(g->steer_lo, g->speed_lo); k->hi = make_double2(g->steer_hi, g->speed_hi);
+    k->lambda = g->lambda; k->seed = g->seed;
+    k->M = g->M; k->K = g->K; k->H = g->H;
+    return true;
+}
+
+int f110_mppi_sample(const f110_sim *sim, const f110_mppi *mppi, const f110_episodes *ep, double *actions, void *stream) {
+    MppiK k;
+    if (!mppi_ok(mppi, &k) || !sim || !sim->steer_cnt || !actions) return F110_ERR_INVALID;
+    if (sim->num_envs <= 0 || sim->num_agents <= 0 || (long long)sim->num_envs * sim->num_agents > 0x7fffffffll)
+        return F110_ERR_INVALID;
+    if (ep && (!ep->terminated || !ep->truncated)) return F110_ERR_INVALID;
+    const long long n = (long long)k.M * k.K * k.H;
+    k_mppi_sample<<<(unsigned)((n + F110_MPPI_SAMPLE_THREADS - 1) / F110_MPPI_SAMPLE_THREADS), F110_MPPI_SAMPLE_THREADS, 0,
+                    (cudaStream_t)stream>>>(k, sim->steer_cnt, ep ? ep->terminated : nullptr, ep ? ep->truncated : nullptr,
+                                            sim->num_envs * sim->num_agents, sim->num_agents,
+                                            reinterpret_cast<double2 *>(actions));
+    LAUNCH_CHECK("k_mppi_sample");
+    return F110_OK;
+}
+
+int f110_mppi_update(const f110_mppi *mppi, const double *actions, const double *cost, double *action_out, int32_t num_rows,
+                     double *weights, int32_t *argmin, void *stream) {
+    MppiK k;
+    if (!mppi_ok(mppi, &k) || !actions || !cost || !action_out || num_rows < 1) return F110_ERR_INVALID;
+    const size_t smem = ((size_t)k.K + 2 * (size_t)k.H) * sizeof(double);     // with the static part <= 48 KiB (mppi.cuh)
+    k_mppi_update<<<(unsigned)k.M, F110_MPPI_UPDATE_THREADS, smem, (cudaStream_t)stream>>>(
+        k, reinterpret_cast<const double2 *>(actions), cost, reinterpret_cast<double2 *>(action_out), num_rows, weights, argmin);
+    LAUNCH_CHECK("k_mppi_update");
     return F110_OK;
 }
 

@@ -62,6 +62,32 @@ __device__ __forceinline__ TrackHit track_search(const double *__restrict__ rec,
     return h;
 }
 
+// track_search in one thread: the same per-segment statements over k = 0 .. W-1 in order, the first minimum kept.  For a
+// caller whose lanes each track a pose of their own (k_scored_rollout).
+__device__ __forceinline__ TrackHit track_search_thread(const double *__restrict__ rec, int n, int base, int W, double px,
+                                                        double py) {
+    double bd = INFINITY, bt = 0.0;
+    int bk = 0x7fffffff;
+    for (int k = 0; k < W; k++) {
+        int i = base + k;
+        if (i >= n) i -= n;
+        const double2 *r = reinterpret_cast<const double2 *>(rec + (size_t)i * F110_TRACK_REC);
+        const double2 xy = __ldg(r), dxy = __ldg(r + 1);
+        const double l2 = __ldg(rec + (size_t)i * F110_TRACK_REC + 4);
+        const double dot = __fma_rn(py - xy.y, dxy.y, (px - xy.x) * dxy.x);     // np.dot: see the top of this file
+        double t = dot / l2;
+        if (t < 0.0) t = 0.0;
+        if (t > 1.0) t = 1.0;
+        const double qx = xy.x + t * dxy.x, qy = xy.y + t * dxy.y;
+        const double ex = px - qx, ey = py - qy;
+        const double d = sqrt(ex * ex + ey * ey);
+        if (d < bd) { bd = d; bt = t; bk = k; }
+    }
+    TrackHit h;
+    h.dist = bd; h.t = bt; h.k = bk;
+    return h;
+}
+
 struct TrackOut {
     double t, dist, s, d, e;
 };

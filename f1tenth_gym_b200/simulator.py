@@ -28,6 +28,11 @@ from . import param_draw as pdraw
 RENDER_MAX_AGENTS = 64     # csrc/render.cuh F110_RENDER_MAX_AGENTS: car quads a block of k_render_views caches
 RENDER_MAX_SIZE = 8192     # largest view height / width of f110_render_views
 TRACK_MAX_WINDOW = 1024    # csrc/progress.cuh F110_TRACK_MAX_WINDOW: largest back + fwd + 1 of the progress tracker
+# The cost weights of predict(cost=) and MPPIPlanner when none are given (include/f110_mppi.h f110_cost): metres, radians and
+# commands per step, progress in metres over the horizon.  The closed-loop test of tests/test_gpu_mppi.py drives with them
+# (DESIGN §3.15 has the sweep they were picked from).
+COST_DEFAULTS = {'w_lat': 1.0, 'w_head': 1.0, 'w_clear': 20.0, 'clear_min': 0.5, 'w_dsteer': 1.0, 'w_dspeed': 0.01,
+                 'w_prog': 10.0, 'w_wall': 1000.0}
 PACKED_RANGE_LIMIT = 32.0  # f110_pack_scans_u24: 24 bits of 2^-19 m clamp every range at 32 m - 2^-19
 
 
@@ -1149,7 +1154,7 @@ class Simulator(object):
         return out
 
     # ------------------------------------------------------------------ predicted futures
-    def predict(self, actions, agent_ids=None, record_states=False, record_clearance=False):
+    def predict(self, actions, agent_ids=None, record_states=False, record_clearance=False, cost=None, prev_action=None):
         """K candidate futures of M agents, H ticks each, in one launch (C ABI f110_predict, include/f110_predict.h), for
         sampling-based control (MPPI, CEM, random shooting).  actions: (M, K, H, 2) fp64 (steer, speed) per step; agent_ids:
         the M flat source agents e*A + slot (repeats allowed), None = every agent (M = N*A).  Sample (m, k) starts from agent
@@ -1164,8 +1169,19 @@ class Simulator(object):
         Ids given on the host are range-checked (ValueError); a CUDA int32 tensor goes to the kernel unchecked, and an id
         outside [0, N*A) there gives NaN states, wall_step -1 and NaN clearance.  ValueError before any device work for a
         bad shape, dtype, device or size, and for a map on which the held-action short path cannot run (no lean ray march,
-        side distances unknown or not below max_range)."""
+        side distances unknown or not below max_range).
+
+        cost: a dict of cost weights (C ABI f110_predict_scored, include/f110_mppi.h) -- any of w_lat, w_head, w_clear, w_dsteer,
+        w_dspeed, w_prog, w_wall (finite, >= 0) and clear_min (metres, finite); missing keys take COST_DEFAULTS -- adds
+        'cost' (M, K) fp64: per step h, w_lat * d^2 + w_head * e^2 + w_clear * max(0, clear_min - clearance)^2 + w_dsteer *
+        (change of steer command)^2 + w_dspeed * (change of speed command)^2, minus w_prog times the progress along the
+        centerline after the last step, plus w_wall when the wall check fired.  d, e and the progress are those of the
+        set_centerlines tracker (its window and reacquire_dist) started at the source agent's pose; the other outputs are
+        unchanged.  prev_action (M, 2): the command before step 0, for the rate terms of step 0 (None: no rate terms there).
+        NaN for a sample whose tracker loses the centerline or whose source is invalid.  ValueError before any device work
+        without centerlines, for an unknown key, a bad weight or a bad prev_action."""
         NA = self.num_envs * self.num_agents
+        cost_c = None if cost is None else self._cost_struct(cost)
         if self.map is None:
             raise ValueError('predict needs a map: call set_map or set_device_map first')
         mc, bc = self._map_struct, self.beams.c
@@ -1203,7 +1219,14 @@ class Simulator(object):
         if M < 1 or K < 1 or not 1 <= H <= nat.PREDICT_MAX_H or M * K > 0x7fffffff:
             raise ValueError('predict needs M >= 1, K >= 1, 1 <= H <= %d and M * K < 2^31, got M=%d K=%d H=%d'
                              % (nat.PREDICT_MAX_H, M, K, H))
-        key = (M, K, H, bool(record_states), bool(record_clearance))
+        prev = None
+        if prev_action is not None:
+            if cost is None:
+                raise ValueError('prev_action is an input of the cost: pass cost as well')
+            prev = torch.as_tensor(prev_action, dtype=torch.float64).to(self.device).contiguous()
+            if tuple(prev.shape) != (M, 2):
+                raise ValueError('prev_action must have shape (M, 2) = (%d, 2), got %s' % (M, tuple(prev.shape)))
+        key = (M, K, H, bool(record_states), bool(record_clearance), cost is not None)
         buf = getattr(self, '_predict_buf', None)
         if buf is None or buf['key'] != key:
             dev = self.device
@@ -1213,6 +1236,10 @@ class Simulator(object):
                    'states': torch.empty((M, K, H, 7), dtype=torch.float64, device=dev) if record_states else None,
                    'clearance': torch.empty((M, K, H), dtype=torch.float32, device=dev) if record_clearance else None,
                    'ids': torch.empty((M,), dtype=torch.int32, device=dev), 'actions': None}
+            if cost is not None:
+                buf['cost'] = torch.empty((M, K), dtype=torch.float64, device=dev)
+                buf['seg0'] = torch.empty((M,), dtype=torch.int32, device=dev)
+                buf['s0'] = torch.empty((M,), dtype=torch.float64, device=dev)
             self._predict_buf = buf
         if ids is None:
             buf['ids'].copy_(torch.from_numpy(a.astype(np.int32)), non_blocking=True)
@@ -1224,17 +1251,51 @@ class Simulator(object):
             act = buf['actions']
         args = nat.F110PredictArgs(nat.ptr(ids), nat.ptr(act), M, K, H, nat.ptr(buf['final_state']), nat.ptr(buf['wall_step']),
                                    nat.ptr(buf['states']), nat.ptr(buf['clearance']))
-        rc = nat.lib().f110_predict(C.byref(self.c), C.byref(mc), C.byref(self._march_tables), C.byref(bc), C.byref(args),
-                                    _stream_ptr(self.device))
+        if cost_c is None:
+            rc = nat.lib().f110_predict(C.byref(self.c), C.byref(mc), C.byref(self._march_tables), C.byref(bc), C.byref(args),
+                                        _stream_ptr(self.device))
+        else:
+            cost_c.prev_action, cost_c.cost, cost_c.seg0, cost_c.s0 = (nat.ptr(prev), nat.ptr(buf['cost']), nat.ptr(buf['seg0']),
+                                                                       nat.ptr(buf['s0']))
+            rc = nat.lib().f110_predict_scored(C.byref(self.c), C.byref(mc), C.byref(self._march_tables), C.byref(bc),
+                                               C.byref(self.centerlines.c), C.byref(args), C.byref(cost_c),
+                                               _stream_ptr(self.device))
         if rc == -1:        # F110_ERR_INVALID: nothing was enqueued
             raise ValueError('f110_predict refused this simulator, map or beam setup (see include/f110_predict.h)')
         nat.check(rc)
         out = {'final_state': buf['final_state'], 'wall_step': buf['wall_step']}
+        if cost is not None:
+            out['cost'] = buf['cost']
         if record_states:
             out['states'] = buf['states']
         if record_clearance:
             out['clearance'] = buf['clearance']
         return out
+
+    def _cost_struct(self, cost):
+        """f110_cost from a dict of weights (missing keys: COST_DEFAULTS) and the tracker settings of set_centerlines; the
+        pointers are left for the caller.  ValueError without centerlines, for an unknown key or a bad value."""
+        if self.centerlines is None:
+            raise ValueError('a cost needs centerlines: call set_centerlines first')
+        if not isinstance(cost, dict):
+            raise ValueError('cost must be a dict of weights, got %r' % (type(cost).__name__,))
+        unknown = set(cost) - set(COST_DEFAULTS)
+        if unknown:
+            raise ValueError('unknown cost keys %s (known: %s)' % (sorted(unknown), sorted(COST_DEFAULTS)))
+        w = dict(COST_DEFAULTS)
+        for k, v in cost.items():
+            try:
+                w[k] = float(v)
+            except (TypeError, ValueError):
+                raise ValueError('cost %s must be a number, got %r' % (k, v))
+            if not np.isfinite(w[k]) or (k != 'clear_min' and w[k] < 0.0):
+                raise ValueError('cost %s must be finite%s, got %r' % (k, '' if k == 'clear_min' else ' and >= 0', v))
+        pc = self._progress_c
+        c = nat.F110Cost()
+        for k in nat.COST_WEIGHTS + ('clear_min',):
+            setattr(c, k, w[k])
+        c.back, c.fwd, c.reacquire_dist = pc.back, pc.fwd, pc.reacquire_dist
+        return c
 
     # ------------------------------------------------------------------ views
     def render_views(self, agent_ids=None, size=(64, 64), metres_per_pixel=0.1, forward_offset=0.0, heading_up=True,
